@@ -5,9 +5,10 @@
   python bench.py --impl reference --gpus N --steps K ...    # the reference's CPU path (C++ restatement) on the host cores
   python bench.py --config 4|5 [--scaling strong]            # the other BASELINE.json sweep configs (default: 2 = configs[1])
   python bench.py --config 3                                 # admission replay: 64-request micro-batches x 200 constraints
+  python bench.py --dump-outputs DIR                         # also write the last timed step's bitmaps and totals as DIR/*.npy
 
 Workload (config.workload), default: BASELINE.json configs[1] -- "audit sweep: 10 templates, 50 constraints, 1M synthetic
-Pods on 1 B200".  Weak scaling: every rank evaluates its own 1M-Pod shard of the cluster and the violation bitmaps are
+Pods on 1 GPU".  Weak scaling: every rank evaluates its own 1M-Pod shard of the cluster and the violation bitmaps are
 exchanged once per step (the one exchange the path has, SURVEY.md 8(e)); `--scaling strong` keeps the total at --objects.
 
 One step = one pass of the hot path over the batch: the fused match-prefilter + predicate kernel over the column-wise batch
@@ -31,7 +32,7 @@ sys.path.insert(0, ROOT)
 
 METRIC = "constraint_object_evals_per_sec_audit_sweep"
 UNIT = "evals/s"
-L2_BYTES = 126 * 1024 * 1024
+DUMP_BUDGET = 60 * 1024 * 1024   # bytes of .npy written by --dump-outputs
 
 
 def env_int(k, d):
@@ -43,7 +44,7 @@ def env_int(k, d):
 
 # ------------------------------------------------------------------------------------------------ clocks
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -195,6 +196,22 @@ def run_reference(args):
     return 0
 
 
+def dump_outputs(out_dir, viol, err, tot, C):
+    """What the timed step hands its caller: the violation and matcher-error bitmaps (one row of uint32 words per object,
+    bit c of word c // 32 = constraint c) and the per-constraint totals ([violations, errors] x constraint), as float64
+    (exact for every uint32 word and every count below 2**53).  A bitmap larger than the budget is reduced to a fixed,
+    seeded sample of rows; rows.npy lists the object indices either way."""
+    import numpy as np
+    n, words = viol.shape
+    keep = min(n, DUMP_BUDGET // (16 * words + 8))
+    rows = np.arange(n) if keep == n else np.sort(np.random.default_rng(0).choice(n, keep, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "violations.npy"), viol[rows].view(np.uint32).astype(np.float64))
+    np.save(os.path.join(out_dir, "errors.npy"), err[rows].view(np.uint32).astype(np.float64))
+    np.save(os.path.join(out_dir, "totals.npy"), tot[:, :C].astype(np.float64))
+
+
 # ------------------------------------------------------------------------------------------------ GPU arm: audit sweeps
 def run_ours(args):
     import numpy as np
@@ -239,7 +256,8 @@ def run_ours(args):
 
     from gatekeeper_b200.sweep import ShardedSweep
     sweep = ShardedSweep(drv, rb, n, C, dev, world)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev) if alg_in < 2 * L2_BYTES else None
+    l2_bytes = torch.cuda.get_device_properties(dev).L2_cache_size
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev) if alg_in < 2 * l2_bytes else None
     ep = D.AUDIT_EP
     stream = torch.cuda.current_stream()
 
@@ -273,6 +291,9 @@ def run_ours(args):
         step(e0[k], e1[k])
     ev_b.record(stream)
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:               # the last timed step's results, before anything below overwrites them
+        shard = sweep.gathered[0].view(n, words) if world > 1 else sweep.viol
+        dumped = (shard.cpu().numpy(), sweep.err.cpu().numpy(), sweep.tot.cpu().numpy())
     if world > 1:
         dist.barrier()
     total_ms = ev_a.elapsed_time(ev_b)
@@ -403,18 +424,11 @@ def run_ours(args):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "data sheet (H100 SXM HBM3, not measured)"
     achieved = alg_bytes / (kern_ms / 1e3) / 1e9
     # gk_spec_kernel: CUDA C++ generated from the constraint set's netlist, compiled by NVRTC at the first large batch (outside the
     # timed region); the netlist interpreter gk_eval_kernel is launched behind it for the tiles it hands over (none on this workload)
     kernel_name = drv.last_kernel()
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tp) and args.config == 2:
-        try:
-            traffic = json.load(open(tp)).get(drv.last_kernel(), {}).get("dram_bytes_per_launch")   # (one ncu --set full capture per kernel)
-        except Exception:
-            traffic = None
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W_,
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None, "dtype": "int (u32 ids / u8 bytes / i64)",
@@ -426,7 +440,7 @@ def run_ours(args):
                                     if sweep.p2p is not None else "one NCCL all-gather (bitmap shard + totals)")) if world > 1 else "single GPU",
                    "violating_pairs_per_step": int(sum(totals_host)), "violating_density": round(sum(totals_host) / max(1, world * n * C), 4),
                    "synth_s": round(gen_s, 2), "ingest_ms_once": round(rb.stats["flatten_ms"] + rb.stats["h2d_ms"], 1), "spot_check": spot},
-        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                      "kernel": kernel_name, "kernel_ms": kern_ms, "alg_bytes_per_launch": alg_bytes, "peak_source": peak_src},
         "e2e": dict(e2e, with_messages=e2e_msgs, audit=e2e_audit), "gpu_launches": int(launches), "clocks": clocks,
     }
@@ -434,6 +448,8 @@ def run_ours(args):
         line["cpu_baseline"] = cpu_baseline(args.config, args.cpu_sample)
     if os.environ.get("GK_BENCH_NOTE"):
         line["note"] = os.environ["GK_BENCH_NOTE"]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, *dumped, C)
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
@@ -479,7 +495,7 @@ def run_admission(args):
     sampler = ClockSampler(0)
     sampler.start()
     lat, kern = [], []
-    K = max(args.steps, 50)
+    K = args.steps
     t_all = time.perf_counter()
     for k in range(K):
         arr, nb, _keep = marshalled[k % len(marshalled)]
@@ -523,7 +539,13 @@ def main():
     ap.add_argument("--msg-sample", type=int, default=50_000, help="objects of the sample whose messages are all rendered (e2e.with_messages)")
     ap.add_argument("--spot-check", type=int, default=300, help="objects of the shard checked against the Python oracle inside the run")
     ap.add_argument("--ref-objects-per-step", type=int, default=40_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed (violation / error bitmaps, totals) "
+                    "as DIR/<name>.npy, float64, at most 60 MB (a fixed, seeded sample of rows beyond that)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl == "reference" or args.config == 3):
+        ap.error("--dump-outputs applies to the audit-sweep workloads (--config 2, 4, 5) of this implementation")
     if args.impl == "reference":
         sys.exit(run_reference(args))
     if args.config == 3:

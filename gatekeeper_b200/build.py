@@ -1,6 +1,6 @@
 """In-tree build of the native libraries (no JIT cache: the .so files travel with the repo snapshot).
 
-  gatekeeper_b200/libgk_engine.so   -- the product: C++ host engine + CUDA kernels for sm_100a (nvcc)
+  gatekeeper_b200/libgk_engine.so   -- the product: C++ host engine + CUDA kernels for sm_90a (nvcc)
   tests/_hostemu/libgk_hostemu.so   -- TEST-ONLY: same host engine linked against the CPU emulation backend
   gatekeeper_b200/libgk_synth.so    -- deterministic synthetic workload generator (bench / tests), not part of the engine
 """
@@ -21,7 +21,7 @@ EMU = os.path.join(ROOT, "tests", "_hostemu", "libgk_hostemu.so")
 HOST_SRCS = ["val.cpp", "rego_parse.cpp", "rego_eval.cpp", "lower.cpp", "xprog.cpp", "expansion.cpp", "engine.cpp", "audit.cpp", "capi.cpp", "coalescer.cpp", "spec_codegen.cpp"]
 SYNTH = os.path.join(ROOT, "gatekeeper_b200", "libgk_synth.so")
 CXXFLAGS = ["-std=c++17", "-O2", "-g1", "-fPIC", "-Wall", "-Wextra", "-pthread", "-I", OBJ]
-NVCCFLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC"]
+NVCCFLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 
 def _nvcc():

@@ -98,8 +98,8 @@ GK_HD int gk_tape_build(const uint8_t* js, uint32_t n, gk_u64* tape, uint32_t ca
   bool in_str = false;                 // between the quotes of a string that started at byte s
   uint32_t s = 0, esc = 0;
   *ntape = 0;
-  // (A warp vote at the head of the loop -- every thread of the warp taking its turns together -- was measured: 12.75 ms per
-  // page against 11.86 ms without; the threads diverge INSIDE a turn, between the alternatives of the token step.)
+  // (A warp vote at the head of the loop -- every thread of the warp taking its turns together -- measured slower than none:
+  // the threads diverge INSIDE a turn, between the alternatives of the token step.)
   while (rc < 0) {
     const bool in_obj = depth > 0 && ((objmask >> (depth - 1)) & 1ull) != 0ull;
     if (in_str) {

@@ -167,7 +167,7 @@ __global__ void __launch_bounds__(256) gk_gvk_minmax_kernel(const unsigned long 
 }
 
 // small host -> device transfers done by the SMs from mapped page-locked memory: they do not queue behind the next page's 32 MB
-// chunks on the copy engine (a 100 KB table upload waited 12 ms there)
+// chunks on the copy engine (a 100 KB table upload waited behind them there)
 __global__ void __launch_bounds__(256) gk_push_kernel(uint8_t* dst, const uint8_t* src, size_t n) {
   const size_t stride = (size_t)gridDim.x * blockDim.x * 16u;
   const bool vec = (reinterpret_cast<size_t>(dst) & 15u) == 0u;

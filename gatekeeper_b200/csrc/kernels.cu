@@ -1,4 +1,4 @@
-// CUDA backend for sm_100a: device memory management, uploads and launches around the tile kernel
+// CUDA backend for sm_90a: device memory management, uploads and launches around the tile kernel
 // (tile_kernel.cuh).  Host <-> device transfers are staged through pinned memory on a private stream; the
 // kernel itself can also be launched on a caller-provided stream into caller-owned device buffers (multi-GPU
 // gather path, where torch.distributed owns the buffers).
@@ -59,7 +59,7 @@ class CudaBackend : public Backend {
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0)
-      throw BackendError{"no CUDA device: gatekeeper_b200 has no CPU fallback; the evaluation path requires a B200 (sm_100a) GPU"};
+      throw BackendError{"no CUDA device: gatekeeper_b200 has no CPU fallback; the evaluation path requires an H100 (sm_90a) GPU"};
     if (device_ >= ndev) throw BackendError{"CUDA device index out of range"};
     CK(cudaSetDevice(device_));
     cudaDeviceProp prop;
@@ -70,9 +70,9 @@ class CudaBackend : public Backend {
     CK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
     {
-      // The tokeniser of the NEXT page runs on a high-priority stream: its launches are small (405 CTAs per 32 MB chunk, 15 % of
-      // the warp slots) and would otherwise only start in the tails of the current page's extraction kernels, whose grids
-      // keep the block scheduler busy -- measured as fully serialised (12.5 + 11.9 = 24.4 ms per page).
+      // The tokeniser of the NEXT page runs on a high-priority stream: its launches are small (a few hundred CTAs per 32 MB
+      // chunk) and would otherwise only start in the tails of the current page's extraction kernels, whose grids keep the
+      // block scheduler busy -- the two pages then run fully serialised.
       int lo = 0, hi = 0;
       CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
       const bool prio = !getenv("GK_NO_STREAM_PRIORITY");
@@ -114,7 +114,7 @@ class CudaBackend : public Backend {
     cudaEventDestroy(ev1_);
     cudaStreamDestroy(stream_);
   }
-  const char* name() const override { return "cuda-sm100a"; }
+  const char* name() const override { return "cuda-sm90a"; }
   const char* last_kernel() const override { return last_kernel_; }
 
   void set_program(const Compiled& c) override {
@@ -190,7 +190,7 @@ class CudaBackend : public Backend {
     // ---- tiling: first row of every scope for every tile, slot offsets from the per-scope tile capacities
     const uint32_t NS = (uint32_t)c.schema.scopes.size();
     // Tile size: kTile objects.  (Shrinking tiles so that the tile count fills whole waves of resident CTAs -- 480 instead
-    // of 512 objects for 1M -- measured slower: 0.816 vs 0.762 ms; the per-tile fixed cost outweighs the fuller last wave.)
+    // of 512 objects for 1M -- measured slower: the per-tile fixed cost outweighs the fuller last wave.)
     uint32_t tile = kTile;
     if (const char* ft = getenv("GK_FORCE_TILE")) tile = std::min<uint32_t>(kTile, std::max(32, atoi(ft)) / 32 * 32);
     uint32_t ntiles = 0;
@@ -555,7 +555,7 @@ class CudaBackend : public Backend {
         std::string tok;
         while (in >> tok) extra.push_back(tok);
       }
-      std::vector<const char*> opts = {"--gpu-architecture=sm_100a", "-std=c++17", "-lineinfo", "-default-device", threads.c_str(), minb.c_str()};
+      std::vector<const char*> opts = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device", threads.c_str(), minb.c_str()};
       for (auto& x : extra) opts.push_back(x.c_str());
       const int rc = compile(prog, (int)opts.size(), opts.data());
       if (rc != 0) {
@@ -1251,9 +1251,9 @@ class CudaBackend : public Backend {
     f.n = nn;
     // H2D of the raw JSON in chunks on the copy stream; the tokeniser of a chunk starts as soon as its bytes have landed
     CK(cudaMemcpyAsync(d + o_ooff, ooff, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, copy_stream_));
-    // Chunk size: a tokeniser launch of a 32 MB chunk (50k Pods) fills 17 % of the warp slots and takes ~0.6 ms whatever its size
-    // (one thread walks one object); bigger chunks mean fewer, fuller launches at the price of a later start.  GK_INGEST_CHUNK_MB
-    // overrides (8 MB chunks measured 85 ms per page instead of 19).
+    // Chunk size: a tokeniser launch of a 32 MB chunk (50k Pods) fills a small share of the warp slots and takes about the same
+    // time whatever its size (one thread walks one object); bigger chunks mean fewer, fuller launches at the price of a later
+    // start, much smaller ones multiply the page time.  GK_INGEST_CHUNK_MB overrides.
     static const size_t kChunk = []() {
       size_t mb = 32;
       if (const char* ev = getenv("GK_INGEST_CHUNK_MB")) mb = (size_t)std::max(1, atoi(ev));
@@ -1356,7 +1356,7 @@ class CudaBackend : public Backend {
   std::vector<cudaEvent_t> chunk_evs_;
   size_t chunk_ev_next_ = 0;
   int device_;
-  int sms_ = 148;
+  int sms_ = 132;
   size_t max_smem_ = 0, sm_smem_ = 0;
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev0_ = nullptr, ev1_ = nullptr;
@@ -1385,7 +1385,7 @@ class CudaBackend : public Backend {
   SpecEntry* spec_cur_ = nullptr;
   bool spec_on_ = !(getenv("GK_SPEC") && atoi(getenv("GK_SPEC")) == 0);
   uint32_t spec_min_objects_ = getenv("GK_SPEC_MIN_OBJECTS") ? (uint32_t)atoll(getenv("GK_SPEC_MIN_OBJECTS")) : 8192u;   // below: not worth a ~2 s NVRTC run
-  // one thread per object of a 512-object tile, 128 registers: the fastest of the shapes measured (profiles/experiments/README.md)
+  // one thread per object of a 512-object tile, 128 registers: the fastest of the shapes measured
   int spec_threads_ = getenv("GK_SPEC_THREADS") ? std::min(1024, std::max(32, atoi(getenv("GK_SPEC_THREADS")) / 32 * 32)) : 512;
   int spec_minb_ = getenv("GK_SPEC_MINB") ? std::max(1, atoi(getenv("GK_SPEC_MINB"))) : 1;
   const char* last_kernel_ = "gk_eval_kernel";

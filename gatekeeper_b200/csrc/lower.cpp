@@ -2569,9 +2569,9 @@ void NetBuilder::build(const std::vector<FP>& formulas, const std::vector<uint32
       ColAtoms& ca = kv.second;
       // Atoms that test a row's type / sid / number (everything but the prefix / suffix / contains tests, which walk the 32-byte
       // HEAD record or the byte pool) CAN be fused per column: one GK_N_ATOMS op loads the column slice once per trip -- four
-      // 32-row groups into registers -- and evaluates every atom of the column on them.  Measured on B200 (round 2, 64 registers,
-      // 4 CTAs per SM, no spills): 0.93 ms per 1M objects fused vs 0.80 ms one op per atom -- fewer instructions per atom, but
-      // 25 long items per tile balance worse over the CTA's 8 warps than 100 short ones.  Off unless GK_FUSED_ATOMS=1.
+      // 32-row groups into registers -- and evaluates every atom of the column on them.  Fusing was slower than
+      // one op per atom -- fewer instructions per atom, but 25 long items per tile balance worse over the CTA's 8 warps than
+      // 100 short ones.  Off unless GK_FUSED_ATOMS=1.
       static const bool fuse = getenv("GK_FUSED_ATOMS") && atoi(getenv("GK_FUSED_ATOMS")) == 1;
       std::vector<GkOp> fused;
       for (auto& a : ca.ops) {

@@ -665,7 +665,7 @@ struct uint4 { uint32_t x, y, z, w; };
     const int P = c.schema.scopes[s].parent;
     o << "  const uint32_t* __restrict__ o" << s << " = scopes[" << s << "].off;\n";
     // (a scope with more rows than a mask holds counts as EMPTY from here on and raises `big`: no branch -- an early return here keeps
-    // every other load of the object waiting behind the three dependent levels of CSR offsets: 0.71-0.73 vs 0.685 ms)
+    // every other load of the object waiting behind the three dependent levels of CSR offsets, which measured slower)
     o << "  const uint32_t lo" << s << " = GK_SPEC_LD(o" << s << " + lo" << P << "), r" << s << " = GK_SPEC_LD(o" << s << " + hi" << P << ") - lo" << s << ";\n";
     o << "  const uint32_t n" << s << " = r" << s << " > 32u ? 0u : r" << s << ", hi" << s << " = lo" << s << " + n" << s << ";\n";
     o << "  const uint32_t f" << s << " = n" << s << " >= 32u ? 0xffffffffu : ((1u << n" << s << ") - 1u);\n  (void)hi" << s << "; (void)f" << s << ";\n  big = big || r" << s
@@ -711,8 +711,8 @@ struct uint4 { uint32_t x, y, z, w; };
   }
   std::sort(order.begin(), order.end());
   // ---- atom groups: ONE row loop per scope computes every atom of that scope (~45 mask registers of the container scope alive at
-  // once, some spilled).  A loop per (scope, template kind) keeps fewer masks alive and measured no better on B200 (0.726 vs 0.719 ms
-  // at 1 M Pods x 50 constraints): every extra loop is one more exposed memory latency per object (profiles/experiments/README.md).
+  // once, some spilled).  A loop per (scope, template kind) keeps fewer masks alive and measured no better: every extra loop is one
+  // more exposed memory latency per object.
   std::map<uint32_t, int> group_ix;   // scope -> row loop
   std::vector<std::vector<uint32_t>> groups;
   for (const Ord& e : order) {

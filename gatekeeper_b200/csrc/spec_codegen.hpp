@@ -4,7 +4,7 @@
 // op a work item some warp decodes, ~400 warp-instructions per object at the benchmark's 50 constraints.  The netlist is known when
 // the constraint set is compiled, so the engine also writes it out as straight-line code -- one thread per object, every node a
 // 32-bit mask register (bit j = row j of THIS object in the node's scope), constants as immediates, EXISTS a `!= 0`, the
-// object-major bitmap words assembled in registers without a transpose -- and NVRTC compiles that text for sm_100a when the first
+// object-major bitmap words assembled in registers without a transpose -- and NVRTC compiles that text for sm_90a when the first
 // large batch is evaluated (kernels.cu).  Objects with more than 32 rows in some scope do not fit the mask registers: their tiles
 // are handed to the interpreter (GkKParams::tile_list).
 #pragma once

@@ -1,4 +1,4 @@
-// The evaluation kernel for sm_100a: a tile-at-a-time columnar bitmap engine.
+// The evaluation kernel for sm_90a: a tile-at-a-time columnar bitmap engine.
 //
 //   * ALL constraints are one netlist of bit-column ops (program.h GkOp).  A CTA owns a tile of kTile consecutive
 //     objects; every node of the netlist is a packed bit column of the tile held in shared memory (32 rows/word).
@@ -70,7 +70,7 @@ using KParams = GkKParams;
 #define GK_THREADS 256
 #endif
 #ifndef GK_TABLES_IN_SMEM
-#define GK_TABLES_IN_SMEM 1   /* measured: 0.825 ms (tables staged in shared memory) vs 0.858 ms (read through L1) per 1M objects */
+#define GK_TABLES_IN_SMEM 1   /* measured: tables staged in shared memory beat reading them through L1 */
 #endif
 #ifndef GK_TILE
 #define GK_TILE 512

@@ -1,4 +1,4 @@
-/* gk_engine.h -- C ABI of the B200 constraint-evaluation engine.
+/* gk_engine.h -- C ABI of the H100 constraint-evaluation engine.
  *
  * This is the boundary a Go `drivers.Driver` shim binds with cgo (see INTEGRATION.md and go/gpudriver/).
  * Each entry point names the reference interface it stands behind (paths relative to the gatekeeper repo):
@@ -101,7 +101,7 @@ gk_engine_t* gk_engine_create(const gk_cfg* cfg, char** err);
 void gk_engine_destroy(gk_engine_t* e);
 const char* gk_backend_name(gk_engine_t* e);
 /* Which kernel decided the engine's last evaluation: "gk_spec_kernel" (CUDA C++ generated from the constraint set's netlist and
- * compiled by NVRTC for sm_100a the first time a batch of >= GK_SPEC_MIN_OBJECTS objects meets the set; GK_SPEC=0 turns it off)
+ * compiled by NVRTC for sm_90a the first time a batch of >= GK_SPEC_MIN_OBJECTS objects meets the set; GK_SPEC=0 turns it off)
  * or "gk_eval_kernel" (the netlist interpreter: small batches, and tiles holding an object with more than 32 rows in a scope).
  * Replaces nothing in the reference: frameworks' rego driver compiles a template's Rego once per AddTemplate
  * (pkg/drivers/k8scel/driver.go:79-146 is the CEL analogue in this tree); this is the per-constraint-set analogue on the device. */

@@ -13,7 +13,7 @@ HOSTEMU = os.path.join(ROOT, "tests", "_hostemu", "libgk_hostemu.so")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
 
 
 @pytest.fixture(scope="session", autouse=True)

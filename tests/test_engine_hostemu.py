@@ -362,7 +362,7 @@ def test_generated_kernel_text_matches_the_interpreted_netlist(config):
 
 
 @pytest.mark.parametrize("config", [2, 4, 5])
-def test_generated_kernel_text_compiles_with_nvrtc_for_sm100a(config, tmp_path, monkeypatch):
+def test_generated_kernel_text_compiles_with_nvrtc_for_sm90a(config, tmp_path, monkeypatch):
     """The text NVRTC gets on the GPU box (kernels.cu: spec_compile, same options) must compile here too -- NVRTC needs no
     device -- and the spec.match blocks must be the written-out form (no block left on the generic gk_match())."""
     import importlib.util

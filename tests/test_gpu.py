@@ -1,6 +1,6 @@
 """GPU parity tests: the product library (CUDA kernels, through the C ABI) against the oracle on the same
 seeded inputs, the committed golden fixtures, and size-independent properties at larger sizes.
-Run on the B200 box:  python -m pytest tests -m gpu -x -q"""
+Run on an H100:  python -m pytest tests -m gpu -x -q"""
 import json
 
 import numpy as np
@@ -21,7 +21,7 @@ def _needs_gpu():
     if not has_cuda():
         pytest.fail("GPU tests selected but no CUDA device is visible")
     d = D.Driver()
-    assert d.backend() == "cuda-sm100a"
+    assert d.backend() == "cuda-sm90a"
     d.close()
 
 

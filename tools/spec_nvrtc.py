@@ -28,7 +28,7 @@ def nvrtc_compile(src: bytes, threads=512, minb=1, defs=()):
     prog = ctypes.c_void_p()
     if h.nvrtcCreateProgram(ctypes.byref(prog), src, b"gk_spec_kernel.cu", 0, None, None) != 0:
         raise RuntimeError("nvrtcCreateProgram failed")
-    opts = [b"--gpu-architecture=sm_100a", b"-std=c++17", b"-lineinfo", b"-default-device", b"-DGK_SPEC_THREADS=%d" % threads, b"-DGK_SPEC_MINB=%d" % minb]
+    opts = [b"--gpu-architecture=sm_90a", b"-std=c++17", b"-lineinfo", b"-default-device", b"-DGK_SPEC_THREADS=%d" % threads, b"-DGK_SPEC_MINB=%d" % minb]
     opts += [d.encode() for d in defs]
     arr = (ctypes.c_char_p * len(opts))(*opts)
     t0 = time.time()
