@@ -65,7 +65,7 @@ class CudaBackend : public Backend {
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device_));
     sms_ = prop.multiProcessorCount;
-    max_smem_ = (size_t)prop.sharedMemPerBlockOptin;
+    max_smem_ = optin_smem_ = (size_t)prop.sharedMemPerBlockOptin;
     sm_smem_ = (size_t)prop.sharedMemPerMultiprocessor;
     CK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
@@ -431,6 +431,20 @@ class CudaBackend : public Backend {
     p.list_mode = 0;
     p.pad_ = 0;
     spec_next_ = spec_ready(db->n);   // (an NVRTC run the first time: here, outside the timed region)
+    if (spec_next_) {
+      // The generated kernel stages the largest tile's rows in shared memory: 32 bits per row of a scope that has atoms (more when it
+      // has more than 32), where the interpreter holds one bit per row per live slot.  A scope with many rows in a tile and few atoms
+      // can therefore need more than the device allows while the interpreter fits: that batch is interpreted.
+      spec_smem_ = spec_cur_->src.smem + spec_cur_->src.stage_bytes(db->cap);
+      spec_next_ = spec_smem_ <= spec_cur_->max_smem;
+      spec_per_sm_ = 0;   // resident CTAs per SM: the persistent grid of fire()
+      if (spec_next_ &&
+          cudaOccupancyMaxActiveBlocksPerMultiprocessor(&spec_per_sm_, reinterpret_cast<const void*>(spec_cur_->kern), spec_cur_->threads, spec_smem_) != cudaSuccess) {
+        cudaGetLastError();
+        spec_per_sm_ = spec_minb_;
+      }
+      spec_per_sm_ = std::max(1, spec_per_sm_);
+    }
 #ifdef GK_PHASE_TIMING
     if (!d_timing_) CK(cudaMalloc(&d_timing_, (kMaxPhases + 2 + 16) * 16));
     CK(cudaMemsetAsync(d_timing_, 0, (kMaxPhases + 2 + 16) * 16, st));
@@ -476,7 +490,10 @@ class CudaBackend : public Backend {
       // the interpreter behind it takes the tiles it listed and, in the fused exchange, publishes the totals of both
       SpecEntry& se = *spec_cur_;
       void* args[] = {&p};
-      CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.kern), dim3(p.ntiles), dim3((unsigned)se.threads), args, se.src.smem, st));
+      // persistent CTAs, as many as are resident at once, walk the tiles with a grid stride: the per-CTA set-up (tables, enforcement
+      // mask) is paid once per CTA, and where two or more are resident one CTA's staging overlaps another's object walk
+      const uint32_t spec_grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * spec_per_sm_)));
+      CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.kern), dim3(spec_grid), dim3((unsigned)se.threads), args, spec_smem_, st));
       ++launches_;
       p.list_mode = 1;
       last_kernel_ = "gk_spec_kernel";
@@ -494,6 +511,7 @@ class CudaBackend : public Backend {
     cudaLibrary_t lib = nullptr;
     cudaKernel_t kern = nullptr;
     int threads = 128;
+    size_t max_smem = 0;      // dynamic shared memory the kernel may be launched with (fixed part + the tile's staging area)
     double compile_ms = 0;
   };
   void spec_select(const Compiled& c) {
@@ -574,8 +592,10 @@ class CudaBackend : public Backend {
       CK(cudaLibraryLoadData(&se.lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0));
       CK(cudaLibraryGetKernel(&se.kern, se.lib, "gk_spec_kernel"));
       se.threads = spec_threads_;
-      if (se.src.smem > 48 * 1024)
-        CK(cudaFuncSetAttribute(reinterpret_cast<const void*>(se.kern), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)se.src.smem));
+      cudaFuncAttributes fa;
+      CK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(se.kern)));
+      se.max_smem = optin_smem_ - fa.sharedSizeBytes;
+      CK(cudaFuncSetAttribute(reinterpret_cast<const void*>(se.kern), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)se.max_smem));
       se.state = 1;
     } catch (const BackendError& e) {
       fprintf(stderr, "[gatekeeper_b200] the kernel generated for constraint set %llu could not be built (%s): the netlist interpreter runs instead\n",
@@ -1385,11 +1405,15 @@ class CudaBackend : public Backend {
   SpecEntry* spec_cur_ = nullptr;
   bool spec_on_ = !(getenv("GK_SPEC") && atoi(getenv("GK_SPEC")) == 0);
   uint32_t spec_min_objects_ = getenv("GK_SPEC_MIN_OBJECTS") ? (uint32_t)atoll(getenv("GK_SPEC_MIN_OBJECTS")) : 8192u;   // below: not worth a ~2 s NVRTC run
-  // one thread per object of a 512-object tile, 128 registers: the fastest of the shapes measured
-  int spec_threads_ = getenv("GK_SPEC_THREADS") ? std::min(1024, std::max(32, atoi(getenv("GK_SPEC_THREADS")) / 32 * 32)) : 512;
-  int spec_minb_ = getenv("GK_SPEC_MINB") ? std::max(1, atoi(getenv("GK_SPEC_MINB"))) : 1;
+  // 256 threads walk a 512-object tile (two objects each), at least two CTAs per SM (<= 128 registers) so that one CTA's staging
+  // overlaps another's object walk: the fastest of 512 x 1, 256 x 2 and 256 x 3 over configs 2, 4 and 5 (256 x 3 spills at config 2)
+  int spec_threads_ = getenv("GK_SPEC_THREADS") ? std::min(1024, std::max(32, atoi(getenv("GK_SPEC_THREADS")) / 32 * 32)) : 256;
+  int spec_minb_ = getenv("GK_SPEC_MINB") ? std::max(1, atoi(getenv("GK_SPEC_MINB"))) : 2;
   const char* last_kernel_ = "gk_eval_kernel";
   bool spec_next_ = false;
+  size_t spec_smem_ = 0;      // dynamic shared memory of the next launch of the generated kernel (set with spec_next_)
+  int spec_per_sm_ = 1;       // its resident CTAs per SM at that size
+  size_t optin_smem_ = 0;     // the device's per-CTA shared-memory limit
   void* pinned_ = nullptr;
   size_t pinned_bytes_ = 0;
 };

@@ -62,6 +62,7 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
   uint32_t* s_tot = act + GK_SPEC_W * 32u;
   uint32_t* s_err = s_tot + GK_SPEC_W * 32u;
   uint32_t* actw = s_err + GK_SPEC_W * 32u;   // the enforcement-point mask packed: bit c of word c / 32
+  uint32_t* stg = reinterpret_cast<uint32_t*>(smem + GK_SPEC_STAGE_AT);   // the tile's staged atom bits and offsets (gk_spec_stage)
   {
     const uint4* a = reinterpret_cast<const uint4*>(p.batch.cols);
     uint4* d = reinterpret_cast<uint4*>(cols);
@@ -87,6 +88,11 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
   for (uint32_t w = 0; w < GK_SPEC_W; ++w) tv[w] = te[w] = 0u;
   for (uint32_t t = blockIdx.x; t < p.ntiles; t += gridDim.x) {
     const uint32_t obj0 = t * p.tile, nobj = min(p.tile, p.batch.n - obj0);
+    // phase 1: the tile's rows, every thread of the CTA; phase 2: its objects, one per thread.  (The barrier at the end of the tile
+    // keeps the next tile's staging from overwriting what the last objects of this one still read.)
+    const uint32_t* tl = p.tile_lo + (size_t)t * NS;
+    gk_spec_stage(p.batch, cols, scopes, p.prog.pool, p.prog.cbytes, tl, tl + NS, stg, threadIdx.x, blockDim.x);
+    __syncthreads();
     // An object with more rows in a scope than a mask register holds makes gk_spec_object() return true: the tile is then listed
     // for the interpreter, which evaluates it again and overwrites what this kernel stored for it; its totals are not counted here.
     int big = 0;
@@ -99,7 +105,7 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
 #pragma unroll
       for (uint32_t w = 0; w < GK_SPEC_W; ++w) vw[w] = ew[w] = 0u;
       if (o < nobj) {
-        if (gk_spec_object(p.batch, cols, scopes, p.prog.pool, p.prog.cbytes, actw, p.out, obj0 + o, vw, ew)) big = 1;
+        if (gk_spec_object(p.batch, stg, p.prog.pool, p.prog.cbytes, actw, p.out, obj0 + o, o, vw, ew)) big = 1;
         const size_t at = (size_t)(obj0 + o) * GK_SPEC_W;
 #if GK_SPEC_W == 2
         const uint2 v2 = make_uint2(vw[0], vw[1]);
@@ -155,13 +161,39 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
   }
 }
 #else
-// TEST-ONLY host build (tests/_hostemu, GK_SPEC_CHECK=1): one object; returns 1 when the object does not fit the mask registers
+#include <vector>
+// TEST-ONLY host build (tests/_hostemu, GK_SPEC_CHECK=1): one object; returns 1 when the object does not fit the mask registers.
+// The object's tile (GK_SPEC_HOST_TILE objects; its rows found through the CSR offsets) is staged by the same gk_spec_stage() the
+// kernel runs, with three "threads" striding over its rows, and staged again only when `obj` leaves it (or starts it again).
+#ifndef GK_SPEC_HOST_TILE
+#define GK_SPEC_HOST_TILE 96u
+#endif
 extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint32_t* ew) {
   uint32_t actw[GK_SPEC_W];
   for (uint32_t w = 0; w < GK_SPEC_W; ++w) vw[w] = ew[w] = actw[w] = 0u;
   for (uint32_t c = 0; c < GK_SPEC_C; ++c)
     if (p->active[c]) actw[c >> 5] |= 1u << (c & 31u);
-  return gk_spec_object(p->batch, p->batch.cols, p->batch.scopes, p->prog.pool, p->prog.cbytes, actw, p->out, obj, vw, ew) ? 1 : 0;
+  struct Tile {
+    const void* flags = nullptr;
+    uint32_t n = 0, t = 0xffffffffu;
+    std::vector<uint32_t> lo, hi, stg;
+  };
+  static thread_local Tile k;
+  const GkBatch& B = p->batch;
+  const uint32_t T = GK_SPEC_HOST_TILE, t = obj / T;
+  if (t != k.t || k.flags != (const void*)B.flags || k.n != B.n || obj % T == 0u) {
+    k.lo.assign(GK_SPEC_NS, 0u);
+    k.hi.assign(GK_SPEC_NS, 0u);
+    k.lo[0] = t * T;
+    k.hi[0] = B.n - t * T < T ? B.n : (t + 1u) * T;
+    gk_spec_tile_rows(B.scopes, k.lo.data(), k.hi.data());
+    k.stg.assign(gk_spec_stage_words(k.lo.data(), k.hi.data()), 0xdeadbeefu);   // (poisoned: a word the staging misses shows)
+    for (uint32_t tid = 0; tid < 3u; ++tid) gk_spec_stage(B, B.cols, B.scopes, p->prog.pool, p->prog.cbytes, k.lo.data(), k.hi.data(), k.stg.data(), tid, 3u);
+    k.flags = B.flags;
+    k.n = B.n;
+    k.t = t;
+  }
+  return gk_spec_object(B, k.stg.data(), p->prog.pool, p->prog.cbytes, actw, p->out, obj, obj - t * T, vw, ew) ? 1 : 0;
 }
 #endif
 )GKSRC";
@@ -487,11 +519,12 @@ struct Gen {
   // `rm` = the mask of the children of parent row pj inside the object's rows of scope L, `pb` = the parent row's own bit.  The CSR
   // offsets are monotone, so rm = (rows below the END of pj) & ~(rows below its START), and the start of pj is the end of pj - 1: one
   // load and one mask per turn, carried.  (lo<L> is by definition the offset at lo<P>: the first parent's children start at bit 0.)
+  // q<L> is the tile's slice of the offsets in shared memory, tile-relative (gk_spec_stage).
   // Not unrolled: parents have one to three rows here, the unrolled-by-four body the compiler makes is text that never runs.
   std::string range_loop_head(uint32_t L) {
     const uint32_t P = (uint32_t)c.schema.scopes[L].parent;
     const std::string l = std::to_string(L), p = std::to_string(P);
-    return "  {\n  uint32_t lmp = 0u;\n  _Pragma(\"unroll 1\") for (uint32_t pj = 0; pj < n" + p + "; ++pj) {\n    const uint32_t rb = GK_SPEC_LD(o" + l + " + lo" + p + " + pj + 1u) - lo" + l +
+    return "  {\n  uint32_t lmp = 0u;\n  _Pragma(\"unroll 1\") for (uint32_t pj = 0; pj < n" + p + "; ++pj) {\n    const uint32_t rb = q" + l + "[lo" + p + " + pj + 1u] - lo" + l +
            ";\n    const uint32_t lm = rb >= 32u ? 0xffffffffu : ((1u << rb) - 1u), rm = lm & ~lmp, pb = 1u << pj;\n    lmp = lm;\n    (void)pb;\n";
   }
 
@@ -602,7 +635,7 @@ SpecSource spec_codegen(const Compiled& c) {
   std::ostringstream o;
   o << "// generated by spec_codegen.cpp for constraint-set version " << c.version << ": " << C << " constraints, " << c.ops.size() << " netlist ops\n";
   o << "#define GK_SPEC_C " << C << "u\n#define GK_SPEC_W " << W << "\n";
-  o << "#ifndef GK_SPEC_THREADS\n#define GK_SPEC_THREADS 512\n#endif\n#ifndef GK_SPEC_MINB\n#define GK_SPEC_MINB 1\n#endif\n";
+  o << "#ifndef GK_SPEC_THREADS\n#define GK_SPEC_THREADS 256\n#endif\n#ifndef GK_SPEC_MINB\n#define GK_SPEC_MINB 2\n#endif\n";
   o << "#ifndef GK_SPEC_HOST\n#define GK_LD(p) __ldg(p)   /* pool, cbytes and every batch array are global and read-only here */\n#endif\n";
   o << strip_includes(kSpecHdrProgram) << strip_includes(kSpecHdrVmCore);
   o << R"GKSRC(
@@ -653,23 +686,6 @@ struct uint4 { uint32_t x, y, z, w; };
       << m.name_len << "u, 0u, 0u})\n";
     o << "GK_SPEC_FN int gk_spec_match_" << mid << "(const GkBatch& B, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes, const uint32_t obj) {\n"
       << "  return gk_match(B, pool, cbytes, M" << mid << ", obj);\n}\n";
-  }
-  // returns true when the object has more rows in some scope than a mask holds: its words are then meaningless (the caller
-  // hands the tile to the interpreter, which stores them again; a matcher error may be listed twice, with the same code)
-  o << "\nGK_SPEC_FN bool gk_spec_object(const GkBatch& B, const GkColumn* cols, const GkScope* scopes, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes,\n"
-       "                               const uint32_t* actw, const GkOut& out, const uint32_t obj, uint32_t* vw, uint32_t* ew) {\n";
-  o << "  const uint32_t lo0 = obj, hi0 = obj + 1u, n0 = 1u, f0 = 1u;\n  (void)lo0; (void)hi0; (void)n0; (void)f0; (void)out; (void)pool; (void)cbytes; (void)cols;\n";
-  o << "  const bool skip = (GK_SPEC_LD(B.flags + obj) & GK_F_SKIP) != 0u;\n  (void)skip;\n  bool big = false;\n";
-  for (size_t s = 1; s < NS; ++s) {
-    if (!g.scope_used[s]) continue;
-    const int P = c.schema.scopes[s].parent;
-    o << "  const uint32_t* __restrict__ o" << s << " = scopes[" << s << "].off;\n";
-    // (a scope with more rows than a mask holds counts as EMPTY from here on and raises `big`: no branch -- an early return here keeps
-    // every other load of the object waiting behind the three dependent levels of CSR offsets, which measured slower)
-    o << "  const uint32_t lo" << s << " = GK_SPEC_LD(o" << s << " + lo" << P << "), r" << s << " = GK_SPEC_LD(o" << s << " + hi" << P << ") - lo" << s << ";\n";
-    o << "  const uint32_t n" << s << " = r" << s << " > 32u ? 0u : r" << s << ", hi" << s << " = lo" << s << " + n" << s << ";\n";
-    o << "  const uint32_t f" << s << " = n" << s << " >= 32u ? 0xffffffffu : ((1u << n" << s << ") - 1u);\n  (void)hi" << s << "; (void)f" << s << ";\n  big = big || r" << s
-      << " > 32u;\n";
   }
   // ---- emission order of the constraints: by template kind, then by the scopes their cones touch
   std::vector<std::vector<uint32_t>> cone_atoms(g.nvar);   // variable -> atoms in its cone (memoised)
@@ -730,43 +746,113 @@ struct uint4 { uint32_t x, y, z, w; };
       groups[(size_t)r.group].push_back(ai);
     }
   }
+  // ---- phase 1, gk_spec_stage(): once per tile the whole CTA evaluates the atoms of every row loop on every row of the tile in that
+  // scope -- consecutive rows in consecutive threads, so the column loads are coalesced and independent -- and stores them as packed
+  // bits in shared memory (ceil(atoms / 32) words per row; bit k of word k / 32 = the loop's k-th atom), together with the tile's
+  // slice of every used nested scope's CSR offsets (tile-relative).  The per-tile layout follows from the rows of every scope in the
+  // tile (tile_lo): a header of region offsets, then the regions.  SpecSource::stage lists them so the launch can size the area.
+  std::vector<uint32_t> nested;   // used nested scopes: their offsets are staged
+  for (size_t s = 1; s < NS; ++s)
+    if (g.scope_used[s]) nested.push_back((uint32_t)s);
+  const uint32_t NG = (uint32_t)groups.size(), NR = NG + (uint32_t)nested.size(), data0 = (NR + 3u) & ~3u;
+  auto group_scope = [&](size_t gi) { return g.atoms[groups[gi][0]].scope; };
+  auto group_words = [&](size_t gi) { return (uint32_t)((groups[gi].size() + 31) / 32); };
+  auto parent_of = [&](uint32_t s) { return (uint32_t)c.schema.scopes[s].parent; };
+  for (size_t gi = 0; gi < NG; ++gi) out.stage.push_back({group_scope(gi), group_words(gi), 0u});
+  for (uint32_t s : nested) out.stage.push_back({parent_of(s), 1u, 1u});
+  out.stage_hdr = data0;
+  std::ostringstream lay;   // the per-tile layout: b<s> / c<s> = first row / rows of scope s in the tile, R<g> / Q<s> = region offsets
+  lay << "  const uint32_t b0 = GK_SPEC_LD(tlo), c0 = GK_SPEC_LD(thi) - b0;\n  (void)b0; (void)c0;\n";
+  for (uint32_t s : nested)
+    lay << "  const uint32_t b" << s << " = GK_SPEC_LD(tlo + " << s << "), c" << s << " = GK_SPEC_LD(thi + " << s << ") - b" << s << ";\n  (void)c" << s << ";\n";
+  lay << "  uint32_t at = " << data0 << "u;\n";
+  for (size_t gi = 0; gi < NG; ++gi) lay << "  const uint32_t R" << gi << " = at;\n  at += c" << group_scope(gi) << " * " << group_words(gi) << "u;\n";
+  for (uint32_t s : nested) lay << "  const uint32_t Q" << s << " = at;\n  at += c" << parent_of(s) << " + 1u;\n";
+  o << "\n#ifdef GK_SPEC_HOST\n";
+  o << "static uint32_t gk_spec_stage_words(const uint32_t* tlo, const uint32_t* thi) {\n" << lay.str() << "  return at;\n}\n";
+  o << "static void gk_spec_tile_rows(const GkScope* scopes, uint32_t* tlo, uint32_t* thi) {\n";
+  for (uint32_t s : nested)
+    o << "  tlo[" << s << "] = scopes[" << s << "].off[tlo[" << parent_of(s) << "]];\n  thi[" << s << "] = scopes[" << s << "].off[thi[" << parent_of(s) << "]];\n";
+  o << "}\n#endif\n";
+  o << "GK_SPEC_FN void gk_spec_stage(const GkBatch& B, const GkColumn* cols, const GkScope* scopes, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes,\n"
+       "                              const uint32_t* tlo, const uint32_t* thi, uint32_t* stg, const uint32_t tid, const uint32_t nthr) {\n"
+       "  (void)B; (void)cols; (void)scopes; (void)pool; (void)cbytes;\n";
+  o << lay.str();
+  o << "  if (tid == 0u) {\n";
+  for (size_t gi = 0; gi < NG; ++gi) o << "    stg[" << gi << "] = R" << gi << ";\n";
+  for (size_t j = 0; j < nested.size(); ++j) o << "    stg[" << NG + j << "] = Q" << nested[j] << ";\n";
+  // the offsets of sibling scopes are read at the same parent rows: one item stages all of a parent's children (independent loads)
+  std::map<uint32_t, std::vector<uint32_t>> children;
+  for (uint32_t s : nested) children[parent_of(s)].push_back(s);
+  o << "  }\n  const uint32_t total = 0u";
+  for (size_t gi = 0; gi < NG; ++gi) o << " + c" << group_scope(gi);
+  for (auto& ch : children) o << " + c" << ch.first << " + 1u";
+  o << ";\n  _Pragma(\"unroll 1\") for (uint32_t i = tid; i < total; i += nthr) {\n    uint32_t k = i;\n";
+  for (size_t gi = 0; gi < NG; ++gi) {
+    const std::vector<uint32_t>& members = groups[gi];
+    const uint32_t s = group_scope(gi), AW = group_words(gi);
+    std::map<uint32_t, uint32_t> need;
+    for (uint32_t ai : members)
+      for (auto& kv : g.atoms[ai].need) need[kv.first] |= kv.second;
+    o << "    if (k < c" << s << ") {   // atoms of scope " << s << " (row loop " << gi << ")\n      const size_t row = (size_t)b" << s << " + k;\n";
+    for (auto& kv : need) {
+      const uint32_t ci = kv.first, enc = kv.second;
+      const std::string K = std::to_string(ci);
+      if (enc & GK_ENC_VT) o << "      const uint32_t t" << K << " = GK_SPEC_LD(cols[" << K << "].vt + row);\n";
+      if (enc & GK_ENC_SID) o << "      const uint32_t i" << K << " = GK_SPEC_LD(cols[" << K << "].sid + row);\n";
+      if (enc & GK_ENC_NUM) o << "      const long long n" << K << " = GK_SPEC_LD(reinterpret_cast<const long long*>(cols[" << K << "].num) + row);\n";
+      if (enc & GK_ENC_HEAD)
+        o << "      const uint4* __restrict__ ph" << K << " = reinterpret_cast<const uint4*>(cols[" << K << "].head);\n      const uint4 h" << K << "a = GK_SPEC_LD(ph" << K
+          << " + 2 * row), h" << K << "b = GK_SPEC_LD(ph" << K << " + 2 * row + 1);\n";
+    }
+    o << "      uint32_t";
+    for (uint32_t w = 0; w < AW; ++w) o << (w ? ", a" : " a") << w << " = 0u";
+    o << ";\n";
+    for (size_t m = 0; m < members.size(); ++m) o << "      if (" << g.atoms[members[m]].expr << ") a" << m / 32 << " |= " << hx(1u << (m % 32)) << ";\n";
+    for (uint32_t w = 0; w < AW; ++w) o << "      stg[R" << gi << " + " << AW << "u * k + " << w << "u] = a" << w << ";\n";
+    o << "      continue;\n    }\n    k -= c" << s << ";\n";
+  }
+  for (auto& ch : children) {
+    const uint32_t P = ch.first;
+    o << "    if (k <= c" << P << ") {   // offsets of the children of scope " << P << "\n";
+    for (uint32_t s : ch.second) o << "      const uint32_t x" << s << " = GK_SPEC_LD(scopes[" << s << "].off + b" << P << " + k);\n";
+    for (uint32_t s : ch.second) o << "      stg[Q" << s << " + k] = x" << s << " - b" << s << ";\n";
+    o << "      continue;\n    }\n    k -= c" << P << " + 1u;\n";
+  }
+  o << "  }\n}\n";
+  // ---- phase 2, gk_spec_object(): one thread per object, from shared memory.  Returns true when the object has more rows in some
+  // scope than a mask holds: its words are then meaningless (the caller hands the tile to the interpreter, which stores them again;
+  // a matcher error may be listed twice, with the same code).  `o` is the object's index in the tile, `obj` its index in the batch.
+  o << "\nGK_SPEC_FN bool gk_spec_object(const GkBatch& B, const uint32_t* stg, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes,\n"
+       "                               const uint32_t* actw, const GkOut& out, const uint32_t obj, const uint32_t o, uint32_t* vw, uint32_t* ew) {\n";
+  o << "  const uint32_t lo0 = o, hi0 = o + 1u, n0 = 1u, f0 = 1u;\n  (void)lo0; (void)hi0; (void)n0; (void)f0; (void)out; (void)pool; (void)cbytes; (void)stg;\n";
+  o << "  const bool skip = (GK_SPEC_LD(B.flags + obj) & GK_F_SKIP) != 0u;\n  (void)skip;\n  bool big = false;\n";
+  for (size_t j = 0; j < nested.size(); ++j) {
+    const uint32_t s = nested[j], P = parent_of(s);
+    o << "  const uint32_t* __restrict__ q" << s << " = stg + stg[" << NG + j << "];\n";
+    // (a scope with more rows than a mask holds counts as EMPTY from here on and raises `big`: no branch)
+    o << "  const uint32_t lo" << s << " = q" << s << "[lo" << P << "], r" << s << " = q" << s << "[hi" << P << "] - lo" << s << ";\n";
+    o << "  const uint32_t n" << s << " = r" << s << " > 32u ? 0u : r" << s << ", hi" << s << " = lo" << s << " + n" << s << ";\n";
+    o << "  const uint32_t f" << s << " = n" << s << " >= 32u ? 0xffffffffu : ((1u << n" << s << ") - 1u);\n  (void)hi" << s << "; (void)f" << s << ";\n  big = big || r" << s
+      << " > 32u;\n";
+  }
   std::vector<uint8_t> group_done(groups.size(), 0);
-  std::set<std::string> ptr_declared;
   auto emit_group = [&](int gi) {
     if (gi < 0 || group_done[(size_t)gi]) return;
     group_done[(size_t)gi] = 1;
     const std::vector<uint32_t>& members = groups[(size_t)gi];
-    const uint32_t s = g.atoms[members[0]].scope;
-    std::map<uint32_t, uint32_t> need;
-    for (uint32_t ai : members)
-      for (auto& kv : g.atoms[ai].need) need[kv.first] |= kv.second;
-    o << "  // ---- atoms of scope " << s << " (row loop " << gi << ")\n";
-    auto decl = [&](const std::string& name, const std::string& text) {
-      if (ptr_declared.insert(name).second) o << text;
-    };
-    for (auto& kv : need) {
-      const uint32_t ci = kv.first, enc = kv.second;
-      const std::string K = std::to_string(ci);
-      if (enc & GK_ENC_VT) decl("pt" + K, "  const uint8_t* __restrict__ pt" + K + " = cols[" + K + "].vt;\n");
-      if (enc & GK_ENC_SID) decl("pi" + K, "  const uint32_t* __restrict__ pi" + K + " = cols[" + K + "].sid;\n");
-      if (enc & GK_ENC_NUM) decl("pn" + K, "  const long long* __restrict__ pn" + K + " = reinterpret_cast<const long long*>(cols[" + K + "].num);\n");
-      if (enc & GK_ENC_HEAD) decl("ph" + K, "  const uint4* __restrict__ ph" + K + " = reinterpret_cast<const uint4*>(cols[" + K + "].head);\n");
-    }
+    const uint32_t s = group_scope((size_t)gi), AW = group_words((size_t)gi);
+    o << "  // ---- atoms of scope " << s << " (row loop " << gi << "): the bits gk_spec_stage() left for the object's rows\n";
+    o << "  const uint32_t* __restrict__ a" << gi << " = stg + stg[" << gi << "];\n";
     o << "  uint32_t";
     for (size_t k = 0; k < members.size(); ++k) o << (k ? ", v" : " v") << g.atoms[members[k]].var << " = 0u";
     o << ";\n";
-    if (s == 0) o << "  {\n    const size_t row = obj;\n    const uint32_t bit = 1u;\n";
-    else o << "  _Pragma(\"unroll 1\") for (uint32_t j = 0; j < n" << s << "; ++j) {\n    const size_t row = (size_t)lo" << s << " + j;\n    const uint32_t bit = 1u << j;\n    (void)bit;\n";
-    for (auto& kv : need) {
-      const uint32_t ci = kv.first, enc = kv.second;
-      if (enc & GK_ENC_VT) o << "    const uint32_t t" << ci << " = GK_SPEC_LD(pt" << ci << " + row);\n";
-      if (enc & GK_ENC_SID) o << "    const uint32_t i" << ci << " = GK_SPEC_LD(pi" << ci << " + row);\n";
-      if (enc & GK_ENC_NUM) o << "    const long long n" << ci << " = GK_SPEC_LD(pn" << ci << " + row);\n";
-      if (enc & GK_ENC_HEAD) o << "    const uint4 h" << ci << "a = GK_SPEC_LD(ph" << ci << " + 2 * row), h" << ci << "b = GK_SPEC_LD(ph" << ci << " + 2 * row + 1);\n";
-    }
-    for (uint32_t ai : members) {
-      o << "    if (" << g.atoms[ai].expr << ") v" << g.atoms[ai].var << " |= bit;\n";
-    }
+    if (s == 0) o << "  {\n    const uint32_t row = o;\n    const uint32_t bit = 1u;\n";
+    else o << "  _Pragma(\"unroll 1\") for (uint32_t j = 0; j < n" << s << "; ++j) {\n    const uint32_t row = lo" << s << " + j;\n    const uint32_t bit = 1u << j;\n";
+    o << "    const uint32_t";
+    for (uint32_t w = 0; w < AW; ++w) o << (w ? ", w" : " w") << w << " = a" << gi << "[" << AW << "u * row + " << w << "u]";
+    o << ";\n";
+    for (size_t m = 0; m < members.size(); ++m) o << "    if (w" << m / 32 << " & " << hx(1u << (m % 32)) << ") v" << g.atoms[members[m]].var << " |= bit;\n";
     o << "  }\n";
   };
   // ---- everything else depth-first from the results: a node right after what it reads
@@ -796,11 +882,12 @@ struct uint4 { uint32_t x, y, z, w; };
   // the enforcement-point filter: one packed word per 32 constraints (actw), not a test per constraint
   for (uint32_t w = 0; w < W; ++w) o << "  vw[" << w << "] &= actw[" << w << "];\n  ew[" << w << "] &= actw[" << w << "];\n";
   o << "  return big;\n}\n";
+  auto r16 = [](size_t x) { return (x + 15) / 16 * 16; };
+  out.smem = r16(c.schema.cols.size() * sizeof(GkColumn) + NS * sizeof(GkScope) + 3 * (size_t)W * 32 * 4 + (size_t)W * 4) + 16;
+  o << "#define GK_SPEC_NS " << NS << "u\n#define GK_SPEC_STAGE_AT " << out.smem << "u   /* the staging area's byte offset in dynamic shared memory */\n";
   o << kWrapper;
   out.src = o.str();
   out.words = W;
-  auto r16 = [](size_t x) { return (x + 15) / 16 * 16; };
-  out.smem = r16(c.schema.cols.size() * sizeof(GkColumn) + NS * sizeof(GkScope) + 3 * (size_t)W * 32 * 4 + (size_t)W * 4) + 16;
   out.n_fast = g.n_fast;
   out.n_generic = g.n_generic;
   return out;

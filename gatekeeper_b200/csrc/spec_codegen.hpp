@@ -9,16 +9,29 @@
 // are handed to the interpreter (GkKParams::tile_list).
 #pragma once
 #include <string>
+#include <vector>
 
 #include "engine.hpp"
 
 namespace gk {
 
 struct SpecSource {
-  std::string src;        // one self-contained translation unit: program.h + vm_core.h + gk_spec_object() + gk_spec_kernel
+  std::string src;        // one self-contained translation unit: program.h + vm_core.h + gk_spec_stage() + gk_spec_object() + gk_spec_kernel
   uint32_t words = 1;     // bitmap words per object
-  size_t smem = 0;        // dynamic shared memory of a launch (column / scope tables, enforcement-point mask, totals)
+  size_t smem = 0;        // fixed dynamic shared memory of a launch (column / scope tables, enforcement-point mask, totals)
   size_t n_fast = 0, n_generic = 0;   // atoms emitted as immediates / as calls of the generic gk_atom()
+  // the per-tile staging area behind the fixed part: `hdr` words, then one region per entry of `stage`
+  struct StageRegion {
+    uint32_t scope, per_row, extra;   // words = (rows of `scope` in the tile) * per_row + extra
+  };
+  std::vector<StageRegion> stage;
+  uint32_t stage_hdr = 0;
+  // bytes of the staging area for a batch whose largest tile has cap[s] rows in scope s
+  size_t stage_bytes(const std::vector<uint32_t>& cap) const {
+    size_t w = stage_hdr;
+    for (const StageRegion& r : stage) w += (size_t)(r.scope < cap.size() ? cap[r.scope] : 0u) * r.per_row + r.extra;
+    return w * 4;
+  }
 };
 
 SpecSource spec_codegen(const Compiled& c);

@@ -2,7 +2,7 @@
 print the static picture: registers, spills, SASS instruction count, instructions per source region.  No GPU needed (NVRTC and
 cuobjdump / nvdisasm run in the authoring container); these are static numbers, never a timing.
 
-    python tools/spec_nvrtc.py /tmp/spec/config2.cu [--threads 512] [--minb 1] [--defs "-DGK_SPEC_X_NOMATCH"]
+    python tools/spec_nvrtc.py /tmp/spec/config2.cu [--threads 256] [--minb 2] [--defs "-DGK_SPEC_X_NOMATCH"]
 """
 import argparse
 import collections
@@ -14,7 +14,7 @@ import sys
 import time
 
 
-def nvrtc_compile(src: bytes, threads=512, minb=1, defs=()):
+def nvrtc_compile(src: bytes, threads=256, minb=2, defs=()):
     """-> (cubin bytes, log text, seconds).  Raises RuntimeError with the log when the text does not compile."""
     h = None
     for name in ("libnvrtc.so.12", "/usr/local/cuda/lib64/libnvrtc.so.12", "libnvrtc.so", "/usr/local/cuda/lib64/libnvrtc.so"):
@@ -59,6 +59,7 @@ def static_report(cubin_path: str, cu_path: str):
     src = open(cu_path).read().split("\n")
     start = next(i for i, s in enumerate(src) if "GK_SPEC_FN bool gk_spec_object" in s) + 1
     end = next(i for i, s in enumerate(src) if s.startswith("#ifndef GK_SPEC_HOST") and i > start)
+    stage = next((i for i, s in enumerate(src) if "GK_SPEC_FN void gk_spec_stage" in s), start) + 1
     cur = None
     region = collections.Counter()
     total = 0
@@ -71,8 +72,9 @@ def static_report(cubin_path: str, cu_path: str):
             total += 1
             if cur is None:
                 region["?"] += 1
+            elif stage <= cur < start:
+                region["stage: atom bits and offsets of the tile's rows (phase 1)"] += 1
             elif cur < start:
-                s = src[cur - 1] if cur <= len(src) else ""
                 region["spec.match (written-out blocks / vm_core.h)"] += 1
             elif cur < end:
                 s = src[cur - 1].strip()
@@ -80,7 +82,7 @@ def static_report(cubin_path: str, cu_path: str):
                     region["object: EXISTS / broadcast range loops"] += 1
                 elif s.startswith("if (") and "|= bit" in s:
                     region["object: atom tests"] += 1
-                elif "GK_SPEC_LD(p" in s or "_Pragma" in s or "bit = " in s:
+                elif "GK_SPEC_LD(p" in s or "_Pragma" in s or "bit = " in s or re.search(r"\bw0 = a\d+\[", s):
                     region["object: row loops (loads, control)"] += 1
                 elif "GK_SPEC_MATCH" in s or "GK_SPEC_ERR" in s:
                     region["object: match call sites"] += 1
@@ -96,8 +98,8 @@ def static_report(cubin_path: str, cu_path: str):
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("cu")
-    ap.add_argument("--threads", type=int, default=512)
-    ap.add_argument("--minb", type=int, default=1)
+    ap.add_argument("--threads", type=int, default=256)
+    ap.add_argument("--minb", type=int, default=2)
     ap.add_argument("--defs", default="")
     a = ap.parse_args()
     cubin, log, dt = nvrtc_compile(open(a.cu, "rb").read(), a.threads, a.minb, a.defs.split())
