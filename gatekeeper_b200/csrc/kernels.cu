@@ -152,8 +152,6 @@ class CudaBackend : public Backend {
     prog_.match = d_match_;
     prog_.pool = d_pool_;
     prog_.cbytes = d_cbytes_;
-    nscopes_ = (uint32_t)c.schema.scopes.size();
-    ncols_ = (uint32_t)c.schema.cols.size();
     const uint32_t C = prog_.nconstraints;
     if (d_totals_) cudaFree(d_totals_);
     CK(cudaMalloc(&d_totals_, (size_t)(2 * std::max(C, 1u)) * sizeof(unsigned long long)));
@@ -189,25 +187,23 @@ class CudaBackend : public Backend {
     pack_layout(hb, c, pb, plan);   // offsets only: the bytes are copied once, below, straight into pinned memory
     // ---- tiling: first row of every scope for every tile, slot offsets from the per-scope tile capacities
     const uint32_t NS = (uint32_t)c.schema.scopes.size();
-    // Tile size: kTile objects.  (Shrinking tiles so that the tile count fills whole waves of resident CTAs -- 480 instead
-    // of 512 objects for 1M -- measured slower: the per-tile fixed cost outweighs the fuller last wave.)
-    uint32_t tile = kTile;
-    if (const char* ft = getenv("GK_FORCE_TILE")) tile = std::min<uint32_t>(kTile, std::max(32, atoi(ft)) / 32 * 32);
+    // Tile size: kTile objects unless the page needs smaller tiles.  (Shrinking tiles so that the tile count fills whole waves of
+    // resident CTAs -- 480 instead of 512 objects for 1M -- measured slower: the per-tile fixed cost outweighs the fuller last wave.)
     uint32_t ntiles = 0;
     std::vector<uint32_t> tile_lo, cap;
-    for (;; tile = std::max(32u, tile / 2 / 32 * 32)) {
-      ntiles = (hb.n + tile - 1) / tile;
+    const uint32_t tile = gk_choose_tile(kTile, net_sizes(c), max_smem_, [&](uint32_t per_tile) -> const std::vector<uint32_t>& {
+      ntiles = (hb.n + per_tile - 1) / per_tile;
       tile_lo.assign((size_t)(ntiles + 1) * NS, 0);
       cap.assign(NS, 0);
       for (uint32_t t = 0; t <= ntiles; ++t) {
         uint32_t* lo = &tile_lo[(size_t)t * NS];
-        lo[0] = std::min<uint32_t>(t * tile, hb.n);
+        lo[0] = std::min<uint32_t>(t * per_tile, hb.n);
         for (uint32_t s = 1; s < NS; ++s) lo[s] = hb.scope_off[s][lo[c.schema.scopes[s].parent]];
         if (t)
           for (uint32_t s = 0; s < NS; ++s) cap[s] = std::max(cap[s], lo[s] - tile_lo[(size_t)(t - 1) * NS + s]);
       }
-      if (tile <= 32 || tile_fits(c, cap, tile)) break;   // (a 32-object tile that still does not fit is refused at launch)
-    }
+      return cap;
+    });
     auto* db = new DevBatch();
     db->bytes = gk_align(plan.total);
     db->n = hb.n;
@@ -249,47 +245,30 @@ class CudaBackend : public Backend {
     return db;
   }
 
-  // ---- adaptive tile size: every bit column of a tile lives in the CTA's shared memory, so a page whose objects iterate very
-  // many rows (one Pod with thousands of containers) needs smaller tiles, not a refusal
-  static uint32_t slot_words_of(const Compiled& c, std::vector<uint32_t> cap, uint32_t tile) {
-    cap[0] = tile;
-    uint64_t w = 0;
-    for (size_t i = 0; i < c.slot_level.size(); ++i) w += ((cap[c.slot_level[i]] + 31) / 32 + 1 + 3) & ~3u;
-    return (uint32_t)std::min<uint64_t>(w, 0xffffffffu);
-  }
-  size_t smem_of(const Compiled& c, uint32_t slot_words) const {
-    auto r16 = [](size_t x) { return (x + 15) / 16 * 16; };
-    const size_t C = c.cons_match.size(), NS = c.schema.scopes.size();
-    size_t smem = 3 * r16(C * 4) + 2 * r16(NS * 4) + r16(c.phase_off.size() * 4) + r16((size_t)slot_words * 4) + 64;
-#if GK_TABLES_IN_SMEM
-    smem += r16(C * sizeof(GkOutEnt)) + r16(c.ops.size() * sizeof(GkOp)) + r16(c.items.size() * 4) + r16(c.match.size() * sizeof(GkMatch)) +
-            r16(c.schema.cols.size() * sizeof(GkColumn)) + r16(NS * sizeof(GkScope)) + r16(c.pool.size() * 4) + r16(c.cbytes.size());
-#endif
-    return smem;
-  }
-  bool tile_fits(const Compiled& c, const std::vector<uint32_t>& cap, uint32_t tile) const {
-    const uint32_t sw = slot_words_of(c, cap, tile);
-    if (sw > 0xffffu || smem_of(c, sw) > max_smem_) return false;
-    return !c.amb || (slot_words_of(*c.amb, cap, tile) <= 0xffffu && smem_of(*c.amb, slot_words_of(*c.amb, cap, tile)) <= max_smem_);
+  // what the decision netlist and, for the audit, the ambiguity netlist of `c` need in shared memory (eval_layout.h)
+  static std::vector<GkNetSize> net_sizes(const Compiled& c) {
+    std::vector<GkNetSize> nets;
+    for (const Compiled* k : {&c, c.amb.get()})
+      if (k)
+        nets.push_back({(uint32_t)k->cons_match.size(), (uint32_t)k->schema.scopes.size(), (uint32_t)k->phase_off.size() - 1, (uint32_t)k->ops.size(),
+                        (uint32_t)k->items.size(), (uint32_t)k->match.size(), (uint32_t)k->schema.cols.size(), (uint32_t)k->pool.size(),
+                        (uint32_t)k->cbytes.size(), k->slot_level});
+    return nets;
   }
 
   // slot area of a tile from the per-scope tile capacities; the netlist with slot ids resolved to word offsets; output planes
   void finish_batch(DevBatch* db, const Compiled& c, std::vector<uint32_t> cap) {
     cap[0] = db->tile;
     db->cap = cap;
-    std::vector<uint32_t> slot_off(c.slot_level.size());
-    uint32_t slot_words = 0;
-    for (size_t i = 0; i < slot_off.size(); ++i) {
-      slot_off[i] = slot_words;
-      slot_words += ((cap[c.slot_level[i]] + 31) / 32 + 1 + 3) & ~3u;   // 16-byte aligned, padded: atoms store 4 words at a time
-    }
-    db->slot_words = slot_words;
+    std::vector<uint32_t> slot_off;
+    const uint64_t slot_words = gk_slot_layout(c.slot_level, cap, &slot_off);
+    if (slot_words > 0xffffu) throw BackendError{"slot area exceeds 16-bit word offsets"};
+    db->slot_words = (uint32_t)slot_words;
     // resolve slot ids -> word offsets once per batch: the kernel then addresses slots without a table lookup
     std::vector<GkOp> ops_r = c.ops;
     std::vector<uint32_t> pool_r = c.pool;
     std::vector<GkOutEnt> outs_r = c.outs;
     {
-      if (slot_words > 0xffffu) throw BackendError{"slot area exceeds 16-bit word offsets"};
       std::vector<uint8_t> done(pool_r.size(), 0);
       auto so = [&](uint32_t slot) { return slot < slot_off.size() ? slot_off[slot] : 0u; };
       for (auto& op : ops_r) {
@@ -461,14 +440,9 @@ class CudaBackend : public Backend {
     if (C) CK(cudaMemsetAsync(totals, 0, (size_t)C * sizeof(unsigned long long), st));
     if (C) CK(cudaMemsetAsync(err_totals, 0, (size_t)C * sizeof(unsigned long long), st));
     CK(cudaMemsetAsync(d_scalars_, 0, 64, st));
-    auto r16 = [](size_t x) { return (x + 15) / 16 * 16; };
-    const size_t NS = nscopes_;
-    size_t smem = 3 * r16((size_t)C * 4) + 2 * r16(NS * 4) + r16((size_t)(prog_.nphases + 1) * 4) + r16((size_t)db->slot_words * 4) + 64;
-#if GK_TABLES_IN_SMEM
-    smem += r16((size_t)C * sizeof(GkOutEnt)) + r16((size_t)prog_.nops * sizeof(GkOp)) + r16((size_t)prog_.nitems * 4) +
-            r16((size_t)prog_.nmatch * sizeof(GkMatch)) + r16((size_t)ncols_ * sizeof(GkColumn)) + r16(NS * sizeof(GkScope)) +
-            r16((size_t)prog_.npool * 4) + r16((size_t)prog_.ncbytes);
-#endif
+    // the kernel carves its shared memory with the same call on the same parameters
+    const size_t smem = gk_eval_layout(p.prog.nconstraints, p.batch.nscopes, p.prog.nphases, p.slot_words, p.prog.nops, p.prog.nitems, p.prog.nmatch,
+                                       p.batch.ncols, p.prog.npool, p.prog.ncbytes).total;
     if (smem > max_smem_)
       throw BackendError{"constraint set needs " + std::to_string(smem) + " bytes of shared memory per CTA (limit " + std::to_string(max_smem_) +
                          "): too many live netlist columns for one launch"};
@@ -1138,8 +1112,6 @@ class CudaBackend : public Backend {
       status->assign(n, 0);
       if (n) CK(cudaMemcpyAsync(status->data(), in.status, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
     }
-    uint32_t tile = kTile;
-    if (const char* ft = getenv("GK_FORCE_TILE")) tile = std::min<uint32_t>(kTile, std::max(32, atoi(ft)) / 32 * 32);
     unsigned long long mm[2] = {~0ull, 0ull};
     if (n) {
       gk_gvk_minmax_kernel<<<std::min<uint32_t>(1024u, (n + 255u) / 256u), 256, 0, stream_>>>(out.gvk, n, d_mm);
@@ -1148,18 +1120,18 @@ class CudaBackend : public Backend {
     }
     std::vector<uint32_t> cap(NS, 0);
     uint32_t ntiles = 0;
-    for (;; tile = std::max(32u, tile / 2 / 32 * 32)) {   // (halved until the tile's bit columns fit the CTA's shared memory)
-      ntiles = (n + tile - 1) / tile;
+    const uint32_t tile = gk_choose_tile(kTile, net_sizes(c), max_smem_, [&](uint32_t per_tile) -> const std::vector<uint32_t>& {
+      ntiles = (n + per_tile - 1) / per_tile;
       if (db->d_tile_lo) dfree(db->d_tile_lo), db->d_tile_lo = nullptr;
       dmalloc(&db->d_tile_lo, ((size_t)(ntiles + 1) * NS) * 4 + 64);
       CK(cudaMemsetAsync(d_cap, 0, (size_t)NS * 4, stream_));
-      gk_tiles_kernel<<<(ntiles + 1 + 127) / 128, 128, 0, stream_>>>(xp, out, n, NS, tile, ntiles, db->d_tile_lo, d_cap);
+      gk_tiles_kernel<<<(ntiles + 1 + 127) / 128, 128, 0, stream_>>>(xp, out, n, NS, per_tile, ntiles, db->d_tile_lo, d_cap);
       ++launches_;
       CK(cudaMemcpyAsync(cap.data(), d_cap, (size_t)NS * 4, cudaMemcpyDeviceToHost, stream_));
       CK(cudaStreamSynchronize(stream_));
       CK(cudaGetLastError());
-      if (tile <= 32 || tile_fits(c, cap, tile)) break;
-    }
+      return cap;
+    });
     db->tile = tile;
     db->ntiles = ntiles;
     db->gvk_uniform = mm[1] == 0 || mm[0] == mm[1];
@@ -1384,7 +1356,6 @@ class CudaBackend : public Backend {
   uint64_t version_ = 0, launches_ = 0;
   GkProgram prog_{};
   std::vector<uint32_t> last_active_;
-  uint32_t ncols_ = 0, nscopes_ = 0;
   GkOp* d_ops_ = nullptr;
   uint32_t* d_items_ = nullptr;
   GkOutEnt* d_outs_ = nullptr;

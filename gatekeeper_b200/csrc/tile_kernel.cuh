@@ -17,6 +17,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "eval_layout.h"
 #include "program.h"
 #include "vm_core.h"
 
@@ -68,9 +69,6 @@ using KParams = GkKParams;
 
 #ifndef GK_THREADS
 #define GK_THREADS 256
-#endif
-#ifndef GK_TABLES_IN_SMEM
-#define GK_TABLES_IN_SMEM 1   /* measured: tables staged in shared memory beat reading them through L1 */
 #endif
 #ifndef GK_TILE
 #define GK_TILE 512
@@ -370,41 +368,24 @@ __device__ __noinline__ void atoms_rows(const GkColumn& c, const uint32_t* ent, 
 __global__ void __launch_bounds__(kThreads, GK_MIN_CTAS) gk_eval_kernel(const KParams p) {
   extern __shared__ __align__(16) unsigned char smem[];
   const uint32_t C = p.prog.nconstraints, W = p.out.words, NS = p.batch.nscopes, NP = p.prog.nphases;
-  // ---- shared-memory layout
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    void* q = smem + off;
-    off += (bytes + 15) / 16 * 16;
-    return q;
-  };
-  uint32_t* s_tot = static_cast<uint32_t*>(take((size_t)C * 4));
-  uint32_t* s_err = static_cast<uint32_t*>(take((size_t)C * 4));
-  uint32_t* s_act = static_cast<uint32_t*>(take((size_t)C * 4));
-  uint32_t* s_lo = static_cast<uint32_t*>(take((size_t)NS * 4));
-  uint32_t* s_cnt = static_cast<uint32_t*>(take((size_t)NS * 4));
-  uint32_t* s_poff = static_cast<uint32_t*>(take((size_t)(NP + 1) * 4));
-  uint32_t* slots = static_cast<uint32_t*>(take((size_t)p.slot_words * 4));
-#if GK_TABLES_IN_SMEM
-  GkOutEnt* outs = static_cast<GkOutEnt*>(take((size_t)C * sizeof(GkOutEnt)));
-  GkOp* ops = static_cast<GkOp*>(take((size_t)p.prog.nops * sizeof(GkOp)));
-  uint32_t* items = static_cast<uint32_t*>(take((size_t)p.prog.nitems * 4));
-  GkMatch* match = static_cast<GkMatch*>(take((size_t)p.prog.nmatch * sizeof(GkMatch)));
-  GkColumn* cols = static_cast<GkColumn*>(take((size_t)p.batch.ncols * sizeof(GkColumn)));
-  GkScope* scopes = static_cast<GkScope*>(take((size_t)NS * sizeof(GkScope)));
-  uint32_t* pool = static_cast<uint32_t*>(take((size_t)p.prog.npool * 4));
-  uint8_t* cbytes = static_cast<uint8_t*>(take((size_t)p.prog.ncbytes));
-#else
-  // the program / schema tables stay in global memory: every access is warp-uniform and read-only, so they live in L1
-  // after the first tile, and the shared memory they would occupy buys resident CTAs instead
-  const GkOutEnt* __restrict__ outs = p.prog.outs;
-  const GkOp* __restrict__ ops = p.prog.ops;
-  const uint32_t* __restrict__ items = p.prog.items;
-  const GkMatch* __restrict__ match = p.prog.match;
-  const GkColumn* __restrict__ cols = p.batch.cols;
-  const GkScope* __restrict__ scopes = p.batch.scopes;
-  const uint32_t* __restrict__ pool = p.prog.pool;
-  const uint8_t* __restrict__ cbytes = p.prog.cbytes;
-#endif
+  // ---- shared-memory layout (the launch is sized with the same call: CudaBackend::prepare)
+  const GkEvalLayout L = gk_eval_layout(p.prog.nconstraints, p.batch.nscopes, p.prog.nphases, p.slot_words, p.prog.nops, p.prog.nitems, p.prog.nmatch,
+                                        p.batch.ncols, p.prog.npool, p.prog.ncbytes);
+  uint32_t* s_tot = reinterpret_cast<uint32_t*>(smem + L.s_tot);
+  uint32_t* s_err = reinterpret_cast<uint32_t*>(smem + L.s_err);
+  uint32_t* s_act = reinterpret_cast<uint32_t*>(smem + L.s_act);
+  uint32_t* s_lo = reinterpret_cast<uint32_t*>(smem + L.s_lo);
+  uint32_t* s_cnt = reinterpret_cast<uint32_t*>(smem + L.s_cnt);
+  uint32_t* s_poff = reinterpret_cast<uint32_t*>(smem + L.s_poff);
+  uint32_t* slots = reinterpret_cast<uint32_t*>(smem + L.slots);
+  GkOutEnt* outs = reinterpret_cast<GkOutEnt*>(smem + L.outs);
+  GkOp* ops = reinterpret_cast<GkOp*>(smem + L.ops);
+  uint32_t* items = reinterpret_cast<uint32_t*>(smem + L.items);
+  GkMatch* match = reinterpret_cast<GkMatch*>(smem + L.match);
+  GkColumn* cols = reinterpret_cast<GkColumn*>(smem + L.cols);
+  GkScope* scopes = reinterpret_cast<GkScope*>(smem + L.scopes);
+  uint32_t* pool = reinterpret_cast<uint32_t*>(smem + L.pool);
+  uint8_t* cbytes = reinterpret_cast<uint8_t*>(smem + L.cbytes);
 
   // list mode (behind gk_spec_kernel): only the tiles that kernel left alone, usually none -- then nothing is staged
   const uint32_t ntiles = p.list_mode ? *p.tile_count : p.ntiles;
@@ -414,18 +395,16 @@ __global__ void __launch_bounds__(kThreads, GK_MIN_CTAS) gk_eval_kernel(const KP
     s_act[i] = p.active[i];
   }
   for (uint32_t i = threadIdx.x; i <= NP; i += blockDim.x) s_poff[i] = p.prog.phase_off[i];
-#if GK_TABLES_IN_SMEM
-  if (ntiles) {
-  stage(outs, p.prog.outs, ((size_t)C * sizeof(GkOutEnt) + 15) / 16 * 16);
-  stage(ops, p.prog.ops, ((size_t)p.prog.nops * sizeof(GkOp) + 15) / 16 * 16);
-  stage(items, p.prog.items, ((size_t)p.prog.nitems * 4 + 15) / 16 * 16);
-  stage(match, p.prog.match, ((size_t)p.prog.nmatch * sizeof(GkMatch) + 15) / 16 * 16);
-  stage(cols, p.batch.cols, ((size_t)p.batch.ncols * sizeof(GkColumn) + 15) / 16 * 16);
-  stage(scopes, p.batch.scopes, ((size_t)NS * sizeof(GkScope) + 15) / 16 * 16);
-  stage(pool, p.prog.pool, ((size_t)p.prog.npool * 4 + 15) / 16 * 16);
-  stage(cbytes, p.prog.cbytes, ((size_t)p.prog.ncbytes + 15) / 16 * 16);
+  if (ntiles) {   // the program and schema tables, each its whole padded region
+    stage(outs, p.prog.outs, L.ops - L.outs);
+    stage(ops, p.prog.ops, L.items - L.ops);
+    stage(items, p.prog.items, L.match - L.items);
+    stage(match, p.prog.match, L.cols - L.match);
+    stage(cols, p.batch.cols, L.scopes - L.cols);
+    stage(scopes, p.batch.scopes, L.pool - L.scopes);
+    stage(pool, p.prog.pool, L.cbytes - L.pool);
+    stage(cbytes, p.prog.cbytes, L.end - L.cbytes);
   }
-#endif
   __syncthreads();
 
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
