@@ -157,7 +157,7 @@ class CudaBackend : public Backend {
     CK(cudaMalloc(&d_totals_, (size_t)(2 * std::max(C, 1u)) * sizeof(unsigned long long)));
     if (d_active_) cudaFree(d_active_);
     CK(cudaMalloc(&d_active_, (size_t)std::max(C, 1u) * 4));
-    if (!d_errlist_) CK(cudaMalloc(&d_errlist_, (size_t)kErrCap * 3 * 4));
+    if (!d_errlist_) CK(cudaMalloc(&d_errlist_, (size_t)err_cap_ * 3 * 4));
     last_active_.clear();
     version_ = c.version;
     spec_select(c);
@@ -387,7 +387,7 @@ class CudaBackend : public Backend {
     p.out.err_totals = err_totals;
     p.out.errlist = d_errlist_;
     p.out.errcount = reinterpret_cast<uint32_t*>(d_scalars_);
-    p.out.errcap = kErrCap;
+    p.out.errcap = err_cap_;
     p.out.words = db->words;
     p.active = d_active_;
     p.prog.ops = db->d_ops;      // slot ids resolved for this batch
@@ -592,13 +592,27 @@ class CudaBackend : public Backend {
     unsigned long long* totals = d_totals_;
     unsigned long long* err_totals = d_totals_ + std::max(C, 1u);
     size_t smem = 0;
-    KParams p = prepare(db, active, db->viol, db->err, totals, err_totals, stream_, &smem);
-    CK(cudaStreamSynchronize(stream_));
-    // the event pair brackets exactly the evaluation kernel
-    CK(cudaEventRecord(ev0_, stream_));
-    fire(p, smem, stream_);
-    CK(cudaEventRecord(ev1_, stream_));
-    CK(cudaStreamSynchronize(stream_));
+    uint32_t nerr = 0;
+    for (;;) {
+      KParams p = prepare(db, active, db->viol, db->err, totals, err_totals, stream_, &smem);
+      CK(cudaStreamSynchronize(stream_));
+      // the event pair brackets exactly the evaluation kernel
+      CK(cudaEventRecord(ev0_, stream_));
+      fire(p, smem, stream_);
+      CK(cudaEventRecord(ev1_, stream_));
+      CK(cudaStreamSynchronize(stream_));
+      CK(cudaMemcpy(&nerr, d_scalars_, 4, cudaMemcpyDeviceToHost));
+      if (nerr <= err_cap_) break;
+      // The kernels count every matcher error but store only the first err_cap_ (object, match block, code) triples.  The code of a
+      // dropped one would be lost -- its autoreject message would carry no reason -- so the list grows to the count and the page is
+      // evaluated again.  Rare (a namespaceSelector over ~a million objects without a cached Namespace), so it costs a normal
+      // evaluation nothing.  eval_into() returns no list and needs no second pass.
+      CK(cudaFree(d_errlist_));
+      d_errlist_ = nullptr;
+      err_cap_ = 0;   // (should the allocation fail, the kernels store nothing until a later evaluation grows the list)
+      CK(cudaMalloc(&d_errlist_, (size_t)nerr * 3 * 4));
+      err_cap_ = nerr;
+    }
     CK(cudaEventElapsedTime(&out.kernel_ms, ev0_, ev1_));
 #ifdef GK_PHASE_TIMING
     {
@@ -630,9 +644,6 @@ class CudaBackend : public Backend {
         out.err_totals[c] = t[std::max(C, 1u) + c];
       }
     }
-    uint32_t nerr = 0;
-    CK(cudaMemcpy(&nerr, d_scalars_, 4, cudaMemcpyDeviceToHost));
-    nerr = std::min(nerr, kErrCap);
     out.errlist.resize((size_t)nerr * 3);
     if (nerr) CK(cudaMemcpy(out.errlist.data(), d_errlist_, (size_t)nerr * 12, cudaMemcpyDeviceToHost));
     if (copy_back) {
@@ -1319,7 +1330,6 @@ class CudaBackend : public Backend {
   }
 
  private:
-  static constexpr uint32_t kErrCap = 1u << 20;
   void free_tables() {
     void** ptrs[] = {(void**)&d_outs_, (void**)&d_ops_, (void**)&d_items_, (void**)&d_phase_off_, (void**)&d_match_, (void**)&d_pool_, (void**)&d_cbytes_};
     for (auto pp : ptrs) {
@@ -1369,6 +1379,7 @@ class CudaBackend : public Backend {
   void* d_scalars_ = nullptr;
   unsigned long long* d_totals_ = nullptr;
   uint32_t* d_errlist_ = nullptr;
+  uint32_t err_cap_ = 1u << 20;   // triples d_errlist_ holds; eval() grows it when a page has more matcher errors
   uint32_t* d_active_ = nullptr;
   unsigned long long* d_timing_ = nullptr;
   int host_threads_ = effective_cpus();
