@@ -7,6 +7,7 @@
 #include <thread>
 #include <cstdint>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <utility>
 #include <string>
@@ -94,6 +95,14 @@ class Backend {
   // Device ingest (ingest_core.h): raw JSON blob -> resident columnar batch without a host parse.  `status` receives one
   // GK_ING_* code per object (the caller renders the error text of the rare non-OK ones with the host parser).
   virtual void* ingest(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status) = 0;
+  // Keeping a page's source for a refresh after a constraint change (gk_batch_refresh, GK_F_KEEP_SOURCE).  ingest_keep() is ingest()
+  // that also hands the caller the page's source in *keep; reextract() builds a new batch from it for the program of rq.c without
+  // reading the caller's page (rq.blob / rq.ooff are not read); release_source() frees it.  The CUDA backend keeps the page's device
+  // JSON, offsets and token tape and re-runs only the extraction passes.  These defaults, for a backend whose pages do not stay on a
+  // device (the test-only host emulation), keep a host copy of the page and ingest it again.
+  virtual void* ingest_keep(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status, void** keep);
+  virtual void* reextract(void* source, const IngestReq& rq, IngestStats* st);
+  virtual void release_source(void* source);
   virtual void identity(void* batch, BatchIdentity& out) = 0;
   // A second view of a resident batch for ANOTHER netlist over the same schema (Compiled::amb): shares the columns, owns its
   // own slot-resolved netlist and output planes.  Evaluate it with eval() while the backend holds `other`; release() it before
@@ -108,6 +117,32 @@ class Backend {
 };
 
 Backend* make_backend(int device);   // defined by whichever backend the library links
+
+// the default page source of Backend::ingest_keep: a host copy of the page
+struct HostPageCopy {
+  std::vector<uint8_t> blob;
+  std::vector<unsigned long long> ooff;
+};
+inline void* Backend::ingest_keep(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status, void** keep) {
+  auto src = std::make_unique<HostPageCopy>();
+  src->blob.assign(rq.blob, rq.blob + rq.ooff[rq.n]);
+  src->blob.resize(src->blob.size() + 16, 0);
+  src->ooff.assign(rq.ooff, rq.ooff + rq.n + 1);
+  void* b = ingest(rq, st, status);
+  *keep = src.release();
+  return b;
+}
+inline void* Backend::reextract(void* source, const IngestReq& rq, IngestStats* st) {
+  auto* src = static_cast<HostPageCopy*>(source);
+  if (!src || src->ooff.size() != rq.n + 1) throw BackendError{"device ingest: the kept source is of another page"};
+  IngestReq r = rq;
+  r.blob = src->blob.data();
+  r.ooff = src->ooff.data();
+  r.lut_fill = [&rq, src](const GkMiss* m, size_t k, std::vector<GkLutVal>& out) { rq.lut_fill_from(src->blob.data(), m, k, out); };
+  std::vector<uint32_t> status;
+  return ingest(r, st, &status);
+}
+inline void Backend::release_source(void* source) { delete static_cast<HostPageCopy*>(source); }
 
 // ---- arena packing shared by both backends: every array of a HostBatch laid out contiguously
 struct PackedBatch {

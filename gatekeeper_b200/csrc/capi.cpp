@@ -128,6 +128,11 @@ struct gk_batch {
   uint32_t flags = 0;                  // the upload's flags (the process whose excluder applied): the audit reviews resultants with the same
   uint64_t alg_bytes = 0;
   uint64_t data_version = 0;           // data.inventory as of the flatten (referential snapshots only)
+  std::vector<std::string> excluded;   // the excluder patterns of the upload's process the batch was flattened with
+  // GK_F_KEEP_SOURCE: the page's source (Backend::ingest_keep -- on the GPU its device JSON, offsets and token tape), and the
+  // review-level errors of its objects (they depend on the page alone)
+  void* source = nullptr;
+  std::vector<std::string> source_errors;
   ObjIn obj_in(size_t i) const;
 };
 
@@ -318,8 +323,15 @@ void eval_batch(gk_engine* e, gk_batch* b, const char* ep_c, uint32_t flags, gk_
 
 const char* process_of(uint32_t flags) { return flags & GK_F_PROCESS_AUDIT ? "audit" : flags & GK_F_PROCESS_WEBHOOK ? "webhook" : ""; }
 
+// the excluder patterns a batch uploaded with `flags` is flattened with (none without a process flag)
+std::vector<std::string> excluded_of(gk_engine* e, uint32_t flags) {
+  const std::string process = process_of(flags);
+  return process.empty() ? std::vector<std::string>() : e->eng->excluded_namespaces(process);
+}
+
 void upload_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, const gk_obj* objs, size_t n, uint32_t flags, gk_batch** outb,
                   gk_result* stats) {
+  std::vector<std::string> excluded = excluded_of(e, flags);   // (read before the flatten: a later change makes the batch stale, never current)
   std::vector<ObjIn> ins(n);
   for (size_t i = 0; i < n; ++i) ins[i] = to_in(objs[i]);
   double t0 = now_ms();
@@ -335,6 +347,7 @@ void upload_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, const 
   b->n = hb->n;
   b->flags = flags;
   b->alg_bytes = hb->alg_bytes;
+  b->excluded = std::move(excluded);
   b->objs.assign(objs, objs + n);
   // drop the host column data; keep the small per-object error list
   auto slim = std::make_shared<HostBatch>();
@@ -364,21 +377,17 @@ static std::vector<gk_obj> blob_objs(const char* buf, const uint64_t* off, size_
   return v;
 }
 
-// a blob of plain objects: flattened by the ingest kernels on the device when the compiled snapshot allows it
-void upload_blob(gk_engine* e, const std::shared_ptr<const Compiled>& c, const char* buf, const uint64_t* off, size_t n, uint8_t source, uint32_t flags,
-                 gk_batch** outb, gk_result* stats) {
+bool device_ingest(const Compiled& c, size_t n) {
   static const bool host_only = getenv("GK_NO_DEVICE_INGEST") != nullptr;
-  if (!c->device_ingest || host_only || n == 0 || getenv("GK_NO_DEVICE_INGEST_RUNTIME")) {   // (the runtime switch is for A/B tests)
-    auto v = blob_objs(buf, off, n, source);
-    upload_batch(e, c, v.data(), n, flags, outb, stats);
-    return;
-  }
-  double t0 = now_ms();
-  IngestReq rq = e->eng->ingest_request(c, reinterpret_cast<const uint8_t*>(buf), reinterpret_cast<const unsigned long long*>(off), n, source, process_of(flags));
-  IngestStats ist;
-  std::vector<uint32_t> status;
+  return c.device_ingest && !host_only && n != 0 && !getenv("GK_NO_DEVICE_INGEST_RUNTIME");   // (the runtime switch is for A/B tests)
+}
+
+// A batch ingested on the device, or re-extracted from its kept source (`ist`, `t0`: the ingest's statistics and start); the
+// review-level errors of its objects are `errors` (empty: none).
+std::unique_ptr<gk_batch> blob_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, void* dev, const char* buf, const uint64_t* off, size_t n,
+                                     uint8_t source, uint32_t flags, std::vector<std::string> errors, const IngestStats& ist, double t0, gk_result* stats) {
   auto b = std::make_unique<gk_batch>();
-  b->dev = e->be->ingest(rq, &ist, &status);
+  b->dev = dev;
   b->compiled = c;
   if (c->uses_data) e->eng->data_doc(&b->data_version);
   b->n = (uint32_t)n;
@@ -390,17 +399,7 @@ void upload_blob(gk_engine* e, const std::shared_ptr<const Compiled>& c, const c
   auto slim = std::make_shared<HostBatch>();
   slim->n = (uint32_t)n;
   slim->alg_bytes = ist.alg_bytes;
-  for (size_t i = 0; i < n; ++i)
-    if (status[i] != GK_ING_OK) {
-      if (slim->obj_errors.empty()) slim->obj_errors.assign(n, std::string());   // (left empty when every object is fine)
-      // the rare rejected object: the host parser words the review-level error (bad JSON, not an object, kind missing)
-      std::string err;
-      VP doc = e->eng->review_doc(b->obj_in(i), nullptr, nullptr, nullptr, &err);
-      if (doc && status[i] != GK_ING_NULL) err = "device ingest refused the object (status " + std::to_string(status[i]) + "): JSON nesting deeper than " +
-                                               std::to_string(GK_TAPE_MAX_DEPTH) + " levels or a token longer than 128 MiB";
-      if (!doc && err.empty()) err = "invalid request object";
-      slim->obj_errors[i] = err;
-    }
+  slim->obj_errors = std::move(errors);
   b->host = slim;
   if (stats) {
     stats->flatten_ms = (now_ms() - t0) - ist.h2d_ms;
@@ -410,6 +409,60 @@ void upload_blob(gk_engine* e, const std::shared_ptr<const Compiled>& c, const c
     stats->n_objects = (uint32_t)n;
     stats->n_constraints = (uint32_t)c->cons_match.size();
   }
+  return b;
+}
+
+// a blob of plain objects: flattened by the ingest kernels on the device when the compiled snapshot allows it
+void upload_blob(gk_engine* e, const std::shared_ptr<const Compiled>& c, const char* buf, const uint64_t* off, size_t n, uint8_t source, uint32_t flags,
+                 gk_batch** outb, gk_result* stats) {
+  if (!device_ingest(*c, n)) {
+    auto v = blob_objs(buf, off, n, source);
+    upload_batch(e, c, v.data(), n, flags, outb, stats);
+    (*outb)->blob = buf;   // (the objects of `objs`, as a blob: a later gk_batch_refresh may ingest them on the device)
+    (*outb)->blob_off = off;
+    (*outb)->blob_source = source;
+    return;
+  }
+  double t0 = now_ms();
+  IngestReq rq = e->eng->ingest_request(c, reinterpret_cast<const uint8_t*>(buf), reinterpret_cast<const unsigned long long*>(off), n, source, process_of(flags));
+  IngestStats ist;
+  std::vector<uint32_t> status;
+  void* kept = nullptr;
+  void* dev = (flags & GK_F_KEEP_SOURCE) ? e->be->ingest_keep(rq, &ist, &status, &kept) : e->be->ingest(rq, &ist, &status);
+  std::vector<std::string> errors;
+  for (size_t i = 0; i < n; ++i)
+    if (status[i] != GK_ING_OK) {
+      if (errors.empty()) errors.assign(n, std::string());   // (left empty when every object is fine)
+      // the rare rejected object: the host parser words the review-level error (bad JSON, not an object, kind missing)
+      ObjIn in;
+      in.json = buf + off[i];
+      in.len = (size_t)(off[i + 1] - off[i]);
+      in.source = source;
+      std::string err;
+      VP doc = e->eng->review_doc(in, nullptr, nullptr, nullptr, &err);
+      if (doc && status[i] != GK_ING_NULL) err = "device ingest refused the object (status " + std::to_string(status[i]) + "): JSON nesting deeper than " +
+                                               std::to_string(GK_TAPE_MAX_DEPTH) + " levels or a token longer than 128 MiB";
+      if (!doc && err.empty()) err = "invalid request object";
+      errors[i] = err;
+    }
+  auto b = blob_batch(e, c, dev, buf, off, n, source, flags, errors, ist, t0, stats);
+  b->excluded = rq.excluded;
+  if (kept) {
+    b->source = kept;
+    b->source_errors = std::move(errors);
+  }
+  *outb = b.release();
+}
+
+// gk_batch_refresh of a batch that kept its source, for a snapshot flattened on the device: the extraction passes again, from the
+// page's token tape in HBM -- no copy, no tokeniser, and the caller's blob is not read
+void refresh_from_source(gk_engine* e, const std::shared_ptr<const Compiled>& c, const gk_batch* old, gk_batch** outb, gk_result* stats) {
+  double t0 = now_ms();
+  IngestReq rq = e->eng->ingest_request(c, nullptr, nullptr, old->n, old->blob_source, process_of(old->flags));
+  IngestStats ist;
+  void* dev = e->be->reextract(old->source, rq, &ist);
+  auto b = blob_batch(e, c, dev, old->blob, old->blob_off, old->n, old->blob_source, old->flags, old->source_errors, ist, t0, stats);
+  b->excluded = rq.excluded;
   *outb = b.release();
 }
 
@@ -755,7 +808,7 @@ int gk_review_blob(gk_engine_t* e, const char* buf, const uint64_t* offsets, siz
                       "aggregate the batch with gk_audit_add_batch, which do"};
     auto c = e->eng->compiled();
     ProgramLease lease(e, *c);
-    upload_blob(e, c, buf, offsets, n, source, flags, &b, &stats);
+    upload_blob(e, c, buf, offsets, n, source, flags & ~(uint32_t)GK_F_KEEP_SOURCE, &b, &stats);   // (the batch lives for this call only)
     std::unique_ptr<gk_batch, std::function<void(gk_batch*)>> hold(b, [&](gk_batch* x) {
       e->be->release(x->dev);
       delete x;
@@ -772,7 +825,43 @@ uint64_t gk_batch_alg_bytes(gk_batch_t* b) { return b ? b->alg_bytes : 0; }
 void gk_batch_free(gk_engine_t* e, gk_batch_t* b) {
   if (!e || !b) return;
   guard(nullptr, [&]() { e->be->release(b->dev); });
+  guard(nullptr, [&]() { e->be->release_source(b->source); });
   delete b;
+}
+
+int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err) {
+  if (!e || !b) return GK_ERR_INVALID;
+  if (stats) memset(stats, 0, sizeof *stats);
+  bool rebuilt = false;
+  const int rc = guard(err, [&]() {
+    auto c = e->eng->compiled();
+    const std::vector<std::string> excluded = excluded_of(e, b->flags);
+    uint64_t dv = 0;
+    if (c->uses_data) e->eng->data_doc(&dv);
+    if (c->version == b->compiled->version && excluded == b->excluded && (!c->uses_data || dv == b->data_version)) {
+      if (stats) {
+        stats->alg_bytes = b->alg_bytes;
+        stats->n_objects = b->n;
+        stats->n_constraints = (uint32_t)c->cons_match.size();
+      }
+      return;
+    }
+    ProgramLease lease(e, *c);
+    gk_batch* nb = nullptr;
+    if (!b->blob) upload_batch(e, c, b->objs.data(), b->objs.size(), b->flags, &nb, stats);
+    else if (b->source && device_ingest(*c, b->n)) refresh_from_source(e, c, b, &nb, stats);
+    else upload_blob(e, c, b->blob, b->blob_off, b->n, b->blob_source, b->flags, &nb, stats);
+    // the new columns replace the old ones; a kept source stays with the batch (a batch that had none may have gained one)
+    if (!nb->source) {
+      std::swap(nb->source, b->source);
+      std::swap(nb->source_errors, b->source_errors);
+    }
+    std::swap(*b, *nb);
+    e->be->release(nb->dev);
+    delete nb;
+    rebuilt = true;
+  });
+  return rc == GK_OK && rebuilt ? 1 : rc;
 }
 
 int gk_set_excluded_namespaces(gk_engine_t* e, const char* process, const char* const* patterns, size_t n, char** err) {

@@ -2060,6 +2060,7 @@ IngestReq Engine::ingest_request(const std::shared_ptr<const Compiled>& c, const
     }
     rq.ns = ns_table_;
   }
+  rq.lut_fill_from = [this, c](const uint8_t* b, const GkMiss* m, size_t k, std::vector<GkLutVal>& out) { lut_fill(*c, b, m, k, out); };
   rq.lut_fill = [this, c, blob](const GkMiss* m, size_t k, std::vector<GkLutVal>& out) { lut_fill(*c, blob, m, k, out); };
   return rq;
 }

@@ -8,6 +8,7 @@
 //   gk_cols_kernel        per row of one scope: every other column encoding; lookups through the device hash tables
 //   gk_scan_*             exclusive prefix sums (counts -> CSR offsets), three small kernels for any length
 //   gk_fill_kernel        the host's answers to the miss list -> table slots
+//   gk_gather_kernel      the argument bytes of the miss list, when the host's copy of the page is not at hand (a kept source)
 //   gk_tiles_kernel       first row of every scope for every evaluation tile + the largest tile of each scope
 // Level-synchronous: every kernel after the tokeniser runs ONE step for all rows of ONE scope, so the threads of a warp follow
 // the same path (the per-object walk of the whole scope tree it replaces ran at 1.7 active threads per warp instruction).
@@ -177,6 +178,15 @@ __global__ void __launch_bounds__(256) gk_push_kernel(uint8_t* dst, const uint8_
     } else {
       for (size_t k = i; k < n && k < i + 16u; ++k) dst[k] = src[k];
     }
+  }
+}
+
+// the page's bytes that missed lookups take as arguments, packed for the host (gk_compact_miss_spans): span k = (page offset,
+// destination offset, length)
+__global__ void gk_gather_kernel(uint8_t* dst, const uint8_t* blob, const unsigned long long* spans, uint32_t nspans) {
+  for (uint32_t k = blockIdx.x; k < nspans; k += gridDim.x) {
+    const unsigned long long src = spans[3 * k], to = spans[3 * k + 1], len = spans[3 * k + 2];
+    for (unsigned long long i = threadIdx.x; i < len; i += blockDim.x) dst[to + i] = blob[src + i];
   }
 }
 

@@ -30,6 +30,22 @@ namespace gk {
     if (e_ != cudaSuccess) throw BackendError{std::string("CUDA error: ") + cudaGetErrorString(e_) + " at " #x}; \
   } while (0)
 
+// The host evaluates a missed lookup from its argument spans in the page.  Without the caller's page (reextract), the spans are
+// gathered from the device copy of it into one compact buffer: fills `spans` with a (page offset, buffer offset, length) triple per
+// span, points the records at the buffer and returns its size.
+inline size_t gk_compact_miss_spans(GkMiss* m, size_t n, std::vector<unsigned long long>& spans) {
+  spans.clear();
+  size_t total = 0;
+  for (size_t i = 0; i < n; ++i)
+    for (GkMissArg& a : m[i].args) {
+      if ((a.kind != GK_ARG_JSON && a.kind != GK_ARG_SYNSTR) || a.len == 0) continue;
+      spans.insert(spans.end(), {a.off, (unsigned long long)total, (unsigned long long)a.len});
+      a.off = total;
+      total += a.len;
+    }
+  return total;
+}
+
 struct DevBatch {
   uint8_t* arena = nullptr;
   size_t bytes = 0;
@@ -698,14 +714,73 @@ class CudaBackend : public Backend {
     CK(cudaStreamSynchronize(stream_));
   }
 
-  void* ingest(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status) override {
+  // A page's device JSON, offsets and token tape, kept for reextract(): the allocation of the front buffer the page was ingested
+  // from, which start_front never hands out again (the front allocates a new one).
+  struct KeptSource {
+    uint8_t* buf = nullptr;
+    GkIngestIn in{};                 // blob / ooff / tape / ntape / status pointers into buf, n
+    unsigned long long bytes = 0;    // the page's JSON bytes
+    ~KeptSource() {
+      if (buf) cudaFree(buf);
+    }
+  };
+
+  void* ingest(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status) override { return ingest_page(rq, st, status, nullptr); }
+  void* ingest_keep(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status, void** keep) override { return ingest_page(rq, st, status, keep); }
+
+  // copy (or take the prefetched copy) and tokenise, then extract; with `keep`, the batch's caller receives the front buffer
+  void* ingest_page(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status, void** keep) {
     std::lock_guard<std::mutex> l(ingest_mu_);
     CK(cudaSetDevice(device_));
+    std::unique_ptr<KeptSource> ks;
+    // the front buffer (blob, offsets, tape): the prefetched copy of this page, or copy + tokenise now
+    auto acquire = [&]() {
+      Front* fr = nullptr;
+      {
+        std::lock_guard<std::mutex> fl(front_mu_);
+        for (auto& f : fronts_)
+          if (f.pending && f.host_blob == rq.blob && f.n == rq.n) fr = &f;   // (prefetched)
+        if (!fr) fr = &start_front(rq.blob, rq.ooff, rq.n);
+        fr->pending = false;
+        if (keep) {
+          ks.reset(new KeptSource());
+          ks->buf = fr->buf.p;
+          ks->in = fr->in;
+          ks->bytes = rq.ooff[rq.n];
+          fr->buf = Scratch{};
+        }
+      }
+      CK(cudaStreamWaitEvent(stream_, fr->done, 0));
+      return fr->in;
+    };
+    void* db = extract(rq, acquire, rq.ooff[rq.n], true, st, status);
+    if (keep) *keep = ks.release();
+    return db;
+  }
+
+  void* reextract(void* source, const IngestReq& rq, IngestStats* st) override {
+    std::lock_guard<std::mutex> l(ingest_mu_);
+    CK(cudaSetDevice(device_));
+    auto* ks = static_cast<KeptSource*>(source);
+    if (!ks || ks->in.n != rq.n) throw BackendError{"device ingest: the kept source is of another page"};
+    if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[launch] extraction of %u objects from the kept source: no copy, no tokeniser\n", ks->in.n);
+    return extract(rq, [ks]() { return ks->in; }, ks->bytes, false, st, nullptr);
+  }
+
+  void release_source(void* source) override {
+    if (!source) return;
+    cudaSetDevice(device_);
+    delete static_cast<KeptSource*>(source);
+  }
+
+  // The extraction half of the device ingest: header, scope, column, byte-column and tile passes over the front buffer `acquire`
+  // makes ready on stream_ (its tokeniser finished).  `B`: the page's JSON bytes; `copied`: this call moved the page to the device.
+  void* extract(const IngestReq& rq, const std::function<GkIngestIn()>& acquire, unsigned long long B, bool copied, IngestStats* st,
+                std::vector<uint32_t>* status) {
     const auto T0 = std::chrono::steady_clock::now();
     const XProgHost& xh = *rq.xprog;
     const Compiled& c = *rq.c;
     const uint32_t n = (uint32_t)rq.n, NS = (uint32_t)xh.scopes.size(), NK = xh.ncounters(), NC = (uint32_t)xh.cols.size();
-    const unsigned long long B = rq.ooff[n];
     if (rq.n > 0x7fffff00ull) throw BackendError{"device ingest: more than 2^31 objects in one batch"};
     // ---- lookup tables
     if (sid_.nstrings != rq.strings->size()) {
@@ -780,7 +855,6 @@ class CudaBackend : public Backend {
     xp.nsn_bytes = d_tab + o_nsnbytes;
     xp.excl_off = excl_off;
     xp.excl_n = excl_n;
-    // ---- front buffer (blob, offsets, tape): the prefetched copy of this page, or copy + tokenise now
     uint32_t clanes = 1;
     if (const char* ev = getenv("GK_INGEST_COL_LANES")) clanes = std::max(1, std::min(32, atoi(ev)));
     while (clanes & (clanes - 1)) --clanes;
@@ -790,15 +864,7 @@ class CudaBackend : public Backend {
     CK(cudaEventCreate(&e2));
     CK(cudaEventCreate(&e3));
     CK(cudaEventRecord(e0, stream_));
-    Front* fr = nullptr;
-    {
-      std::lock_guard<std::mutex> fl(front_mu_);
-      for (auto& f : fronts_)
-        if (f.pending && f.host_blob == rq.blob && f.n == rq.n) fr = &f;   // (prefetched)
-      if (!fr) fr = &start_front(rq.blob, rq.ooff, rq.n);
-      fr->pending = false;
-    }
-    CK(cudaStreamWaitEvent(stream_, fr->done, 0));
+    const GkIngestIn src = acquire();
     // ---- back scratch: header counters + scratch flags, totals, scan block sums, miss list, the pointer tables of the count phase
     const uint32_t miss_cap = 1u << 17;
     const uint32_t NT = GK_CNT_EXTRA + NS + xh.nbytecols + 4;          // totals: header counters, scopes, byte columns
@@ -807,7 +873,7 @@ class CudaBackend : public Backend {
                  o_sums = sc.take((size_t)NT * 4096 * 4), o_miss = sc.take((size_t)miss_cap * sizeof(GkMiss)), o_fill = sc.take((size_t)miss_cap * 8),
                  o_prec = sc.take((size_t)NS * 8);
     uint8_t* d_s = scratch_.need(gk_align(sc.off));
-    GkIngestIn in = fr->in;
+    GkIngestIn in = src;
     in.source = rq.source;
     in.counts = reinterpret_cast<uint32_t*>(d_s + o_counts);
     in.misses = reinterpret_cast<GkMiss*>(d_s + o_miss);
@@ -1082,7 +1148,24 @@ class CudaBackend : public Backend {
       hmiss.resize(m);
       CK(cudaMemcpy(hmiss.data(), in.misses, (size_t)m * sizeof(GkMiss), cudaMemcpyDeviceToHost));
       std::vector<GkLutVal> vals;
-      rq.lut_fill(hmiss.data(), m, vals);
+      if (rq.blob) {
+        rq.lut_fill(hmiss.data(), m, vals);
+      } else {   // (reextract: the argument bytes come from the device copy of the page)
+        std::vector<unsigned long long> spans;
+        std::vector<uint8_t> args(gk_compact_miss_spans(hmiss.data(), m, spans) + 1);
+        const uint32_t nspans = (uint32_t)(spans.size() / 3);
+        if (nspans) {
+          auto* d_spans = reinterpret_cast<unsigned long long*>(talloc(spans.size() * 8));
+          uint8_t* d_args = talloc(args.size());
+          CK(cudaMemcpyAsync(d_spans, spans.data(), spans.size() * 8, cudaMemcpyHostToDevice, stream_));
+          gk_gather_kernel<<<std::min<uint32_t>(nspans, 4096u), 128, 0, stream_>>>(d_args, in.blob, d_spans, nspans);
+          ++launches_;
+          CK(cudaMemcpyAsync(args.data(), d_args, args.size() - 1, cudaMemcpyDeviceToHost, stream_));
+          CK(cudaStreamSynchronize(stream_));
+          CK(cudaGetLastError());
+        }
+        rq.lut_fill_from(args.data(), hmiss.data(), m, vals);
+      }
       // append the results, point the claimed slots at them
       const uint32_t base = (uint32_t)lutv_.size();
       lutv_.insert(lutv_.end(), vals.begin(), vals.end());
@@ -1155,7 +1238,7 @@ class CudaBackend : public Backend {
       cudaEventElapsedTime(&ms, e1, e3);
       st->extract_ms = ms - lut_ms;
       st->lut_ms = lut_ms;
-      st->h2d_bytes = B + ((size_t)n + 1) * 8 + tab_bytes + aimg.size();
+      st->h2d_bytes = (copied ? B + ((size_t)n + 1) * 8 : 0) + tab_bytes + aimg.size();
       st->lut_misses = total_miss;
       st->alg_bytes = alg;
       st->launches = launches_;
@@ -1278,6 +1361,7 @@ class CudaBackend : public Backend {
       ++launches_;
       first = last;
     }
+    if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[launch] gk_tape_kernel over %u objects, after a host->device copy of %llu bytes\n", n, B);
     if (n == 0) CK(cudaStreamWaitEvent(front_stream_, chunk_event_after_copy(), 0));
     CK(cudaEventRecord(f.done, front_stream_));
     f.pending = true;

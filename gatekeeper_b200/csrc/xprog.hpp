@@ -82,8 +82,11 @@ struct IngestReq {
   const StringTable* strings = nullptr;
   std::shared_ptr<const NsTableHost> ns;
   std::vector<std::string> excluded;          // excluder patterns of the calling process
-  // host evaluation of the lookups the device missed: one GkLutVal per record, in order
+  // host evaluation of the lookups the device missed: one GkLutVal per record, in order; the records' argument spans are byte
+  // offsets into `blob`
   std::function<void(const GkMiss* misses, size_t n, std::vector<GkLutVal>& out)> lut_fill;
+  // the same with the spans read from `bytes` instead: a refresh from a kept source has no caller's page (Backend::reextract)
+  std::function<void(const uint8_t* bytes, const GkMiss* misses, size_t n, std::vector<GkLutVal>& out)> lut_fill_from;
 };
 
 struct IngestStats {

@@ -25,6 +25,7 @@ GATOR_EP = "gator.gatekeeper.sh"
 SOURCE = {"": 0, None: 0, "Original": 1, "Generated": 2, "All": 3}
 
 F_BITMAP_ONLY, F_MATERIALIZE, F_NO_COPY_BACK = 0, 1, 2
+F_KEEP_SOURCE = 4
 F_PROCESS_AUDIT, F_PROCESS_WEBHOOK = 16, 32
 PROCESS_FLAG = {"": 0, None: 0, "audit": F_PROCESS_AUDIT, "webhook": F_PROCESS_WEBHOOK}
 
@@ -69,7 +70,7 @@ EXPORTS = [
     "gk_constraint_key", "gk_result_constraint_key", "gk_review_batch", "gk_batch_upload", "gk_batch_eval", "gk_batch_eval_device",
     "gk_batch_eval_device_peers", "gk_batch_upload_blob", "gk_review_blob", "gk_set_excluded_namespaces", "gk_audit_begin", "gk_audit_add_batch", "gk_audit_report",
     "gk_audit_end", "gk_validation_messages", "gk_host_cpus", "gk_pin_host", "gk_blob_prefetch", "gk_coalescer_create", "gk_coalescer_review", "gk_coalescer_stats",
-    "gk_coalescer_destroy", "gk_batch_size", "gk_batch_alg_bytes", "gk_batch_free", "gk_free_result", "gk_free_str", "gk_dump",
+    "gk_coalescer_destroy", "gk_batch_size", "gk_batch_alg_bytes", "gk_batch_free", "gk_batch_refresh", "gk_free_result", "gk_free_str", "gk_dump",
     "gk_stat_description",
 ]
 
@@ -141,6 +142,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.gk_batch_alg_bytes.restype = U64
     lib.gk_batch_alg_bytes.argtypes = [P]
     lib.gk_batch_free.argtypes = [P, P]
+    lib.gk_batch_refresh.argtypes = [P, P, C.POINTER(gk_result), PP]
     lib.gk_free_result.argtypes = [C.POINTER(gk_result)]
     lib.gk_free_str.argtypes = [C.c_void_p]
     lib.gk_dump.restype = C.c_void_p
@@ -500,12 +502,14 @@ class Driver:
         err = C.c_char_p()
         self._check(self._lib.gk_blob_prefetch(self._e, blob.buf, blob.offsets, len(blob), C.byref(err)), err)
 
-    def upload_blob(self, blob, source: str = "Original", process: str = ""):
-        """Flatten + upload a page of objects held in one contiguous buffer (workloads.ObjectBlob)."""
+    def upload_blob(self, blob, source: str = "Original", process: str = "", keep_source: bool = False):
+        """Flatten + upload a page of objects held in one contiguous buffer (workloads.ObjectBlob).  keep_source: the batch keeps the
+        page's JSON and token tape on the device, so that ResidentBatch.refresh() re-extracts it without copying it again."""
         h = C.c_void_p()
         stats = gk_result()
         err = C.c_char_p()
-        self._check(self._lib.gk_batch_upload_blob(self._e, blob.buf, blob.offsets, len(blob), SOURCE.get(source, 4), PROCESS_FLAG.get(process, 0), C.byref(h),
+        flags = PROCESS_FLAG.get(process, 0) | (F_KEEP_SOURCE if keep_source else 0)
+        self._check(self._lib.gk_batch_upload_blob(self._e, blob.buf, blob.offsets, len(blob), SOURCE.get(source, 4), flags, C.byref(h),
                                                    C.byref(stats), C.byref(err)), err)
         return ResidentBatch(self, h, blob, {"flatten_ms": stats.flatten_ms, "h2d_ms": stats.h2d_ms, "h2d_bytes": stats.h2d_bytes,
                                              "alg_bytes": stats.alg_bytes})
@@ -642,6 +646,19 @@ class ResidentBatch:
         self.drv._check(self.drv._lib.gk_batch_eval_device_peers(self.drv._e, self.h, enforcement_point.encode(), arr, len(peer_bases), rank,
                                                                  slot_i32, tot_off_i32, tot_stride, d_err, d_totals, d_err_totals, stream,
                                                                  C.byref(err)), err)
+
+    def refresh(self) -> dict:
+        """gk_batch_refresh: bring the batch to the engine's current constraint set (and excluder patterns, and data.inventory) so that
+        eval() accepts it again.  Returns the call's statistics; "rebuilt" is False when the batch was already current."""
+        stats = gk_result()
+        err = C.c_char_p()
+        rc = self.drv._lib.gk_batch_refresh(self.drv._e, self.h, C.byref(stats), C.byref(err))
+        if rc < 0:
+            self.drv._check(rc, err)
+        out = {"flatten_ms": stats.flatten_ms, "h2d_ms": stats.h2d_ms, "h2d_bytes": stats.h2d_bytes, "alg_bytes": stats.alg_bytes}
+        if rc == 1:
+            self.stats = out
+        return dict(out, rebuilt=rc == 1)
 
     def free(self):
         if self.h:

@@ -85,6 +85,20 @@ func (r *AuditRun) AddPage(b *C.gk_batch_t, enforcementPoint string) error {
 	return nil
 }
 
+// RefreshBatch brings a resident batch to the current constraint set, excluder patterns and data.inventory (gk_batch_refresh), so
+// that an audit run can add it again after a template or constraint changed.  A page uploaded with GK_F_KEEP_SOURCE is re-extracted
+// from its token tape in HBM; any other is flattened again from the objects or blob it was uploaded from, which must still be alive.
+// A batch that was already current is left as it is.  On error the batch is unchanged.
+func (d *Driver) RefreshBatch(b *C.gk_batch_t) error {
+	d.mux.RLock()
+	defer d.mux.RUnlock()
+	var cerr *C.char
+	if rc := C.gk_batch_refresh(d.e, b, nil, &cerr); rc < 0 {
+		return takeErr(cerr)
+	}
+	return nil
+}
+
 func (r *AuditRun) Report() (*AuditReport, error) {
 	var cerr *C.char
 	js := C.gk_audit_report(r.a, &cerr)

@@ -44,6 +44,9 @@ enum {
   GK_F_BITMAP_ONLY = 0,      /* violation / error bitmaps + per-constraint totals */
   GK_F_MATERIALIZE = 1,      /* also render {msg, details} for every flagged pair (types.Result list) */
   GK_F_NO_COPY_BACK = 2,     /* leave bitmaps on the device (throughput measurement); totals still returned */
+  /* gk_batch_upload_blob: the batch keeps the page's device JSON, offsets and token tape until gk_batch_free, so that
+   * gk_batch_refresh re-extracts its columns without copying or tokenising the page again (HBM cost: DESIGN.md section 5b) */
+  GK_F_KEEP_SOURCE = 4,
   /* which caller's excluder applies at flatten time (gk_set_excluded_namespaces); neither bit = no excluder stage (gator) */
   GK_F_PROCESS_AUDIT = 16,   /* process.Audit   -- pkg/audit/manager.go:531-538,600 */
   GK_F_PROCESS_WEBHOOK = 32  /* process.Webhook -- pkg/webhook/policy.go:170-178 */
@@ -182,6 +185,15 @@ int gk_review_blob(gk_engine_t* e, const char* buf, const uint64_t* offsets, siz
 uint32_t gk_batch_size(gk_batch_t* b);
 uint64_t gk_batch_alg_bytes(gk_batch_t* b);
 void gk_batch_free(gk_engine_t* e, gk_batch_t* b);
+/* Bring a resident batch to the engine's current constraint set, excluder patterns of the upload's process, and (referential
+ * constraint sets) data.inventory: afterwards it is what a fresh upload of the same objects with the same flags would be, and the
+ * eval and audit calls accept it again.  Every column is extracted again (string ids depend on the engine-wide string table, which
+ * new constraints extend).  A blob batch uploaded with GK_F_KEEP_SOURCE is re-extracted on the device from its kept token tape when
+ * the constraint set is flattened on the device; every other batch is flattened again from the caller's objects or blob, which must
+ * still be alive, as for any resident batch.  Returns 1 when the batch was rebuilt, 0 when it was already current (nothing done),
+ * negative on error -- then the batch is unchanged, still on its old constraint set.  `stats` (may be NULL): flatten_ms, h2d_ms,
+ * h2d_bytes, alg_bytes as for an upload. */
+int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err);
 
 /* ---- stage-0 excluder: Config.spec.match[].excludedNamespaces of one process ("audit", "webhook", "sync",
  * "mutation-webhook", or "*" = all four), pkg/controller/config/process/excluder.go:53-127.  Replaces the process' set.
