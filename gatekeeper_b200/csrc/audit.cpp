@@ -76,6 +76,10 @@ void AuditRun::merge(AuditRun& o) {
   results += o.results;
   rendered_pairs += o.rendered_pairs;
   counted_pairs += o.counted_pairs;
+  for (auto& fe : o.first_object_errors)
+    if (first_object_errors.size() < 20) first_object_errors.emplace_back(seen_objects + fe.first, fe.second);
+  object_errors += o.object_errors;
+  seen_objects += o.seen_objects;
 }
 
 namespace {
@@ -106,19 +110,21 @@ struct IdView {
 }  // namespace
 
 void AuditRun::add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn>& objs, const uint32_t* viol, const uint32_t* err,
-                         uint32_t words, const std::vector<uint32_t>& errlist, const std::string& ep, const BatchIdentity* id, const uint32_t* amb) {
+                         uint32_t words, const std::vector<uint32_t>& errlist, const std::string& ep, const BatchIdentity* id, const uint32_t* amb,
+                         const uint32_t* cand) {
   const size_t n = objs.size();
   const uint32_t C = (uint32_t)c.order.size();
   // ---- lazy path: which pairs need the host at all
-  // cand[c] = the objects whose results can still enter constraint c's list.  Constraints that may have several results per pair
-  // are evaluated for every pair (their totals count results: pkg/audit/manager.go:886-945).
-  const bool lazy = id && id->uniform_gvk && id->flags.size() == n &&
+  // the candidates of c = the objects whose results can still enter constraint c's list.  Constraints that may have several results
+  // per pair are evaluated for every pair (their totals count results: pkg/audit/manager.go:886-945).
+  const bool lazy = (cand || (id && id->uniform_gvk && id->flags.size() == n)) &&
                     (amb || std::any_of(c.single_result.begin(), c.single_result.end(), [](uint8_t x) { return x != 0; }));
+  if (cand) id = nullptr;   // (the candidate bitmap replaces the threshold scan below)
   // exactly one result for a violating pair: proven for the constraint when it was lowered, or for this pair by the ambiguity bitmap
   auto one_result = [&](size_t o, uint32_t cix) { return c.single_result[cix] || (amb && !(amb[o * words + (cix >> 5)] >> (cix & 31u) & 1u)); };
   std::vector<uint32_t> thr_obj(C, 0);     // per single-result constraint: an object holding the limit-th smallest identity
   std::vector<uint8_t> thr_all(C, 1);      // fewer than `limit` flagged objects: all are candidates
-  if (lazy && limit) {
+  if (lazy && limit && !cand) {
     const IdView iv{*id};
     const size_t TT = std::min<size_t>((size_t)std::max(1, eng.threads()), std::max<size_t>(1, n / 4096));
     // per thread, per constraint: max-heap of the `limit` smallest objects seen
@@ -193,8 +199,9 @@ void AuditRun::add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn
               bool is_err = eb >> k & 1u;
               if (lazy && !is_err && one_result(o, cix)) {
                 // one result per pair: counted here; evaluated only if the object can still enter the constraint's list
-                const bool cand = limit && (thr_all[cix] || IdView{*id}.cmp((uint32_t)o, thr_obj[cix]) <= 0);
-                if (!cand) {
+                const bool candidate = limit && (cand ? (cand[o * words + w] >> k & 1u) != 0
+                                                      : (thr_all[cix] || IdView{*id}.cmp((uint32_t)o, thr_obj[cix]) <= 0));
+                if (!candidate) {
                   ++counted[cix];
                   continue;
                 }
@@ -256,6 +263,157 @@ void AuditRun::add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn
     if (!e.empty()) throw RegoError{"audit: " + e};
   for (auto& p : parts) merge(p);
   objects += n;
+}
+
+// Backend::audit_candidates on the host: the flagged objects sorted by (group, version, kind, namespace, name), then per constraint
+// the rank of its limit-th flagged object bounds its candidates.
+void Backend::audit_candidates(void* batch, const uint32_t* viol, uint32_t words, uint32_t nconstraints, uint32_t limit, const GvkOf& gvk_of,
+                               std::vector<uint32_t>& cand, float* device_ms) {
+  if (device_ms) *device_ms = 0.f;
+  BatchIdentity id;
+  identity(batch, id);
+  const size_t n = id.flags.size();
+  cand.assign(n * words, 0u);
+  const IdView iv{id};
+  auto bit = [&](uint32_t o, uint32_t cix) { return (viol[(size_t)o * words + (cix >> 5)] >> (cix & 31u) & 1u) != 0; };
+  struct Flagged {
+    uint32_t o;
+    std::string g, v, k;
+  };
+  std::vector<Flagged> fl;
+  for (uint32_t o = 0; o < n; ++o)
+    for (uint32_t cix = 0; cix < nconstraints; ++cix)
+      if (bit(o, cix)) {
+        fl.push_back({o, {}, {}, {}});
+        gvk_of(o, fl.back().g, fl.back().v, fl.back().k);
+        break;
+      }
+  auto cmp = [&](const Flagged& a, const Flagged& b) {
+    if (a.g != b.g) return a.g < b.g ? -1 : 1;
+    if (a.v != b.v) return a.v < b.v ? -1 : 1;
+    if (a.k != b.k) return a.k < b.k ? -1 : 1;
+    return iv.cmp(a.o, b.o);
+  };
+  std::sort(fl.begin(), fl.end(), [&](const Flagged& a, const Flagged& b) { return cmp(a, b) < 0; });
+  std::vector<uint32_t> rank(fl.size(), 0);
+  for (size_t p = 1; p < fl.size(); ++p) rank[p] = rank[p - 1] + (cmp(fl[p - 1], fl[p]) != 0);
+  for (uint32_t cix = 0; cix < nconstraints; ++cix) {
+    uint32_t seen = 0, thr = ~0u;
+    for (size_t p = 0; p < fl.size() && thr == ~0u; ++p)
+      if (bit(fl[p].o, cix) && ++seen == limit) thr = rank[p];
+    for (size_t p = 0; p < fl.size() && rank[p] <= thr; ++p)
+      if (bit(fl[p].o, cix)) cand[(size_t)fl[p].o * words + (cix >> 5)] |= 1u << (cix & 31u);
+  }
+}
+
+// ---- export / import of a run's partial state (gk_audit_export / gk_audit_merge)
+//   "GKAUDIT\0", u32 format version, the fields in declaration order (integers u64 little-endian, strings as u64 length + bytes),
+//   then an FNV-1a 64 checksum of every byte before it
+namespace {
+constexpr char kRunMagic[8] = {'G', 'K', 'A', 'U', 'D', 'I', 'T', '\0'};
+constexpr uint32_t kRunFormat = 1;
+uint64_t fnv64(const uint8_t* p, size_t n) {
+  uint64_t h = 1469598103934665603ull;
+  for (size_t i = 0; i < n; ++i) h = (h ^ p[i]) * 1099511628211ull;
+  return h;
+}
+struct Writer {
+  std::string s;
+  void u64(uint64_t x) {
+    for (int i = 0; i < 8; ++i) s.push_back((char)(x >> (8 * i) & 0xffu));
+  }
+  void str(const std::string& x) {
+    u64(x.size());
+    s += x;
+  }
+};
+struct Reader {
+  const uint8_t* p;
+  size_t n, at = 0;
+  void need(uint64_t k) {
+    if (k > n - at) throw RegoError{"audit merge: the buffer is truncated"};
+  }
+  uint64_t u64() {
+    need(8);
+    uint64_t x = 0;
+    for (int i = 0; i < 8; ++i) x |= (uint64_t)p[at + i] << (8 * i);
+    at += 8;
+    return x;
+  }
+  std::string str() {
+    const uint64_t k = u64();
+    need(k);
+    std::string x(reinterpret_cast<const char*>(p + at), (size_t)k);
+    at += (size_t)k;
+    return x;
+  }
+  uint64_t count(uint64_t min_bytes_each) {   // an element count that the remaining bytes can hold
+    const uint64_t k = u64();
+    if (min_bytes_each && k > (n - at) / min_bytes_each) throw RegoError{"audit merge: the buffer is truncated"};
+    return k;
+  }
+};
+}  // namespace
+
+std::string AuditRun::serialize() const {
+  Writer w;
+  w.s.assign(kRunMagic, sizeof kRunMagic);
+  for (int i = 0; i < 4; ++i) w.s.push_back((char)(kRunFormat >> (8 * i) & 0xffu));
+  for (uint64_t x : {(uint64_t)limit, (uint64_t)msg_size, objects, results, rendered_pairs, counted_pairs, object_errors, seen_objects}) w.u64(x);
+  w.u64(first_object_errors.size());
+  for (auto& fe : first_object_errors) w.u64(fe.first), w.str(fe.second);
+  w.u64(by_action.size());
+  for (auto& kv : by_action) w.str(kv.first), w.u64(kv.second);
+  w.u64(per_constraint.size());
+  for (auto& kv : per_constraint) {
+    w.str(kv.first);
+    w.u64(kv.second.total);
+    w.u64(kv.second.queue.heap.size());
+    for (auto& sv : kv.second.queue.heap)
+      for (const std::string* f : {&sv.group, &sv.version, &sv.kind, &sv.ns, &sv.name, &sv.message, &sv.action, &sv.scoped_json}) w.str(*f);
+  }
+  w.u64(fnv64(reinterpret_cast<const uint8_t*>(w.s.data()), w.s.size()));
+  return w.s;
+}
+
+AuditRun AuditRun::parse(const uint8_t* buf, size_t len) {
+  if (!buf || len < sizeof kRunMagic + 4 + 8) throw RegoError{"audit merge: the buffer is truncated"};
+  if (memcmp(buf, kRunMagic, sizeof kRunMagic) != 0) throw RegoError{"audit merge: not an exported audit run"};
+  uint32_t format = 0;
+  for (int i = 0; i < 4; ++i) format |= (uint32_t)buf[sizeof kRunMagic + i] << (8 * i);
+  if (format != kRunFormat)
+    throw RegoError{"audit merge: export format " + std::to_string(format) + ", this library reads format " + std::to_string(kRunFormat)};
+  uint64_t sum = 0;
+  for (int i = 0; i < 8; ++i) sum |= (uint64_t)buf[len - 8 + i] << (8 * i);
+  if (sum != fnv64(buf, len - 8)) throw RegoError{"audit merge: checksum mismatch (the buffer is truncated or corrupted)"};
+  Reader r{buf, len - 8, sizeof kRunMagic + 4};
+  AuditRun run;
+  run.limit = (size_t)r.u64();
+  run.msg_size = (size_t)r.u64();
+  run.objects = r.u64(), run.results = r.u64(), run.rendered_pairs = r.u64(), run.counted_pairs = r.u64();
+  run.object_errors = r.u64(), run.seen_objects = r.u64();
+  for (uint64_t i = 0, k = r.count(16); i < k; ++i) {
+    const uint64_t at = r.u64();
+    run.first_object_errors.emplace_back(at, r.str());
+  }
+  for (uint64_t i = 0, k = r.count(16); i < k; ++i) {
+    std::string a = r.str();
+    run.by_action[a] = r.u64();
+  }
+  for (uint64_t i = 0, k = r.count(24); i < k; ++i) {
+    auto& pc = run.per_constraint[r.str()];
+    pc.queue.limit = run.limit;
+    pc.total = r.u64();
+    for (uint64_t j = 0, m = r.count(64); j < m; ++j) {
+      StatusViolation sv;
+      for (std::string* f : {&sv.group, &sv.version, &sv.kind, &sv.ns, &sv.name, &sv.message, &sv.action, &sv.scoped_json}) *f = r.str();
+      pc.queue.heap.push_back(std::move(sv));
+    }
+    if (pc.queue.heap.size() > run.limit || !std::is_heap(pc.queue.heap.begin(), pc.queue.heap.end(), sv_less))
+      throw RegoError{"audit merge: a status list of the buffer is not a limit queue"};
+  }
+  if (r.at != r.n) throw RegoError{"audit merge: trailing bytes after the run"};
+  return run;
 }
 
 static void sv_json(const StatusViolation& sv, std::string& o) {

@@ -43,16 +43,25 @@ struct AuditRun {
   void add_object_errors(const std::vector<std::string>& errs);
 
   void fold(const std::string& key, StatusViolation sv);
+  // `other`'s partial state folded in as if its objects came after this run's (its object-error indices are offset by
+  // seen_objects): merging shard runs in shard order gives the report of one run over the shards in that order
   void merge(AuditRun& other);
   // fold every result of a reviewed batch: viol/err are the kernel's bitmaps [n * words]
-  // `id` (the batch's namespace / name arrays, read back from the device): with it, the pairs of constraints that have one
-  // result per pair (Compiled::single_result) are COUNTED from the bitmap, and only the objects that can still enter a
-  // constraint's list -- the `limit` smallest by (namespace, name), ties included -- are evaluated for their messages.
+  // Lazy path: the pairs of constraints that have one result per pair (Compiled::single_result) are COUNTED from the bitmap, and only
+  // the candidates -- the objects that can still enter a constraint's list -- are evaluated for their messages.  The candidates come
+  // either from `cand` (Backend::audit_candidates: the `limit` smallest by (group, version, kind, namespace, name), any mix of kinds)
+  // or, on a page of one kind, from `id` (the batch's namespace / name arrays: the `limit` smallest by (namespace, name)), ties
+  // included either way.
   void add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn>& objs, const uint32_t* viol, const uint32_t* err,
                  uint32_t words, const std::vector<uint32_t>& errlist, const std::string& ep, const BatchIdentity* id = nullptr,
-                 const uint32_t* amb = nullptr);   // amb: the ambiguity netlist's bitmap (bit clear = at most one result for the pair)
+                 const uint32_t* amb = nullptr,    // amb: the ambiguity netlist's bitmap (bit clear = at most one result for the pair)
+                 const uint32_t* cand = nullptr);  // cand: the candidate bitmap [n * words]
   uint64_t rendered_pairs = 0, counted_pairs = 0;   // pairs evaluated on the host / taken from the bitmap (lazy path)
   std::string report();
+  // The run's partial state as a versioned byte string (gk_audit_export), and its inverse: parse() fills an empty run or throws
+  // RegoError on a truncated, corrupted or foreign buffer.
+  std::string serialize() const;
+  static AuditRun parse(const uint8_t* buf, size_t len);
 };
 
 void validation_messages(const Compiled& c, const std::vector<Violation>& vio, uint32_t object, std::vector<std::string>& deny,

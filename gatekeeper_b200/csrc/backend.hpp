@@ -7,6 +7,7 @@
 #include <thread>
 #include <cstdint>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <new>
 #include <utility>
@@ -104,6 +105,15 @@ class Backend {
   virtual void* reextract(void* source, const IngestReq& rq, IngestStats* st);
   virtual void release_source(void* source);
   virtual void identity(void* batch, BatchIdentity& out) = 0;
+  // The audit's candidates of a reviewed batch for any mix of kinds (gk_audit_add_batch_ordered).  Objects are ordered by (group,
+  // version, kind, namespace, name) as sv_less orders results (namespace and name as BatchIdentity holds them); for constraint c the
+  // candidates are the objects whose bit c is set in `viol` [n * words] and whose identity is at or below the `limit`-th smallest
+  // such identity, ties included (all of them when fewer than `limit` are set).  `cand` receives that bitmap [n * words].  `gvk_of`
+  // decodes the (group, version, kind) of one object from its JSON: the backend asks for one object of each distinct apiVersion /
+  // kind it holds.  The CUDA backend ranks and selects on the device; this default does it on the host from identity().
+  using GvkOf = std::function<void(uint32_t object, std::string& group, std::string& version, std::string& kind)>;
+  virtual void audit_candidates(void* batch, const uint32_t* viol, uint32_t words, uint32_t nconstraints, uint32_t limit, const GvkOf& gvk_of,
+                                std::vector<uint32_t>& cand, float* device_ms);
   // A second view of a resident batch for ANOTHER netlist over the same schema (Compiled::amb): shares the columns, owns its
   // own slot-resolved netlist and output planes.  Evaluate it with eval() while the backend holds `other`; release() it before
   // the batch it was forked from.

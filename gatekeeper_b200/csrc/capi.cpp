@@ -876,6 +876,7 @@ int gk_set_excluded_namespaces(gk_engine_t* e, const char* process, const char* 
 struct gk_audit {
   gk_engine* e;
   AuditRun run;
+  float select_ms = 0.f;   // device time of the last gk_audit_add_batch_ordered's ranking and selection
 };
 
 gk_audit_t* gk_audit_begin(gk_engine_t* e, uint32_t violations_limit, uint32_t msg_size, char** err) {
@@ -889,7 +890,9 @@ gk_audit_t* gk_audit_begin(gk_engine_t* e, uint32_t violations_limit, uint32_t m
   return a;
 }
 
-int gk_audit_add_batch(gk_audit_t* a, gk_batch_t* b, const char* ep_c, char** err) {
+// gk_audit_add_batch and gk_audit_add_batch_ordered: `ordered` takes the lazy path's candidates from Backend::audit_candidates (any mix
+// of kinds) instead of the host threshold scan over (namespace, name), which only a page of one kind allows
+static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordered, char** err) {
   if (!a || !b) return GK_ERR_INVALID;
   return guard(err, [&]() {
     gk_engine* e = a->e;
@@ -914,8 +917,8 @@ int gk_audit_add_batch(gk_audit_t* a, gk_batch_t* b, const char* ep_c, char** er
     // the pairs that have exactly one result and evaluate only what can still enter a constraint's list.
     BatchIdentity id;
     const bool lazy = !getenv("GK_AUDIT_EAGER") && (c->amb || std::any_of(c->single_result.begin(), c->single_result.end(), [](uint8_t x) { return x != 0; }));
-    if (lazy) e->be->identity(b->dev, id);
-    const bool use_amb = lazy && id.uniform_gvk && c->amb && !getenv("GK_AUDIT_NO_AMB");
+    if (lazy && !ordered) e->be->identity(b->dev, id);
+    const bool use_amb = lazy && (ordered || id.uniform_gvk) && c->amb && !getenv("GK_AUDIT_NO_AMB");
     if (use_amb) {
       ProgramLease lease(e, *c->amb);   // (the backend holds one netlist at a time: waits until no review uses the other)
       void* fork = e->be->fork_batch(b->dev, *c->amb);
@@ -973,8 +976,19 @@ int gk_audit_add_batch(gk_audit_t* a, gk_batch_t* b, const char* ep_c, char** er
         }
       for (auto& p : part) children.insert(children.end(), std::make_move_iterator(p.begin()), std::make_move_iterator(p.end()));
     }
-    a->run.add_batch(*e->eng, *c, ins, ev.viol.data(), ev.err.empty() ? nullptr : ev.err.data(), ev.words, ev.errlist, ep, lazy ? &id : nullptr,
-                     use_amb ? ev_amb.viol.data() : nullptr);
+    // (after the expansion above: the rows of objects whose expansion failed are cleared, and they are no candidates either)
+    std::vector<uint32_t> cand;
+    if (lazy && ordered) {
+      auto gvk_of = [&ins](uint32_t o, std::string& g, std::string& v, std::string& k) {
+        try {
+          split_gv(json_parse(ins[o].json, ins[o].len), g, v, k);
+        } catch (JsonError&) {
+        }
+      };
+      e->be->audit_candidates(b->dev, ev.viol.data(), ev.words, (uint32_t)c->order.size(), (uint32_t)a->run.limit, gvk_of, cand, &a->select_ms);
+    }
+    a->run.add_batch(*e->eng, *c, ins, ev.viol.data(), ev.err.empty() ? nullptr : ev.err.data(), ev.words, ev.errlist, ep,
+                     lazy && !ordered ? &id : nullptr, use_amb ? ev_amb.viol.data() : nullptr, lazy && ordered ? cand.data() : nullptr);
     if (!children.empty()) {
       std::vector<gk_obj> cobjs(children.size());
       for (size_t k = 0; k < children.size(); ++k) {
@@ -1037,6 +1051,39 @@ int gk_audit_add_batch(gk_audit_t* a, gk_batch_t* b, const char* ep_c, char** er
     }
     a->run.add_object_errors(obj_errs);
   });
+}
+
+int gk_audit_add_batch(gk_audit_t* a, gk_batch_t* b, const char* ep, char** err) { return audit_add(a, b, ep, false, err); }
+
+int gk_audit_add_batch_ordered(gk_audit_t* a, gk_batch_t* b, const char* ep, char** err) { return audit_add(a, b, ep, true, err); }
+
+float gk_audit_select_ms(gk_audit_t* a) { return a ? a->select_ms : 0.f; }
+
+int gk_audit_export(gk_audit_t* a, char** buf, size_t* len, char** err) {
+  if (!a || !buf || !len) return GK_ERR_INVALID;
+  *buf = nullptr;
+  *len = 0;
+  return guard(err, [&]() {
+    const std::string s = a->run.serialize();
+    char* p = static_cast<char*>(malloc(s.size()));
+    if (!p) throw std::bad_alloc();
+    memcpy(p, s.data(), s.size());
+    *buf = p;
+    *len = s.size();
+  });
+}
+
+int gk_audit_merge(gk_audit_t* a, const char* buf, size_t len, char** err) {
+  if (!a || (!buf && len)) return GK_ERR_INVALID;
+  const int rc = guard(err, [&]() {
+    AuditRun other = AuditRun::parse(reinterpret_cast<const uint8_t*>(buf), len);   // (the run is untouched until the buffer is whole)
+    if (other.limit != a->run.limit || other.msg_size != a->run.msg_size) {
+      throw RegoError{"audit merge: the exported run has violations_limit " + std::to_string(other.limit) + " and msg_size " +
+                      std::to_string(other.msg_size) + ", this run " + std::to_string(a->run.limit) + " and " + std::to_string(a->run.msg_size)};
+    }
+    a->run.merge(other);
+  });
+  return rc == GK_ERR_REGO ? GK_ERR_INVALID : rc;   // (every RegoError here is about the buffer)
 }
 
 char* gk_audit_report(gk_audit_t* a, char** err) {

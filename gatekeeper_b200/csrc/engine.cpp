@@ -1457,6 +1457,7 @@ struct Flattener : ChunkOut {
   void header_row(const VP& o, const VP& ns, uint8_t source, bool present, bool second_row = false) {
     uint32_t fl = 0;
     uint32_t kind = GK_SID_UNDEF, group = GK_SID_UNDEF;
+    uint64_t gvk = 0;
     if (present && o) {
       fl |= GK_F_HAS_OBJ;
       std::string g, v, k;
@@ -1472,6 +1473,7 @@ struct Flattener : ChunkOut {
         hh |= 1ull;
         hb.gvk_lo = std::min(hb.gvk_lo, hh);
         hb.gvk_hi = std::max(hb.gvk_hi, hh);
+        gvk = hh;
       }
       bool is_ns = k == "Namespace" && g.empty();
       if (is_ns) fl |= GK_F_IS_NS;
@@ -1498,6 +1500,7 @@ struct Flattener : ChunkOut {
         }
     }
     fl |= ((uint32_t)source << GK_F_SRC_SHIFT) & GK_F_SRC_MASK;
+    if (!second_row) hb.gvk.push_back(gvk);
     hb.flags.push_back(fl);
     hb.kind_sid.push_back(kind);
     hb.group_sid.push_back(group);
@@ -1543,7 +1546,7 @@ struct Flattener : ChunkOut {
     std::swap(hb.flags, o_flags), std::swap(hb.kind_sid, o_kind), std::swap(hb.group_sid, o_group), std::swap(hb.nsn_off, o_nsn_off), std::swap(hb.nsn_bytes, o_nsn_bytes);
     std::swap(hb.name_off, o_name_off), std::swap(hb.gen_off, o_gen_off), std::swap(hb.lbl_off, o_lbl_off), std::swap(hb.lbl_kv, o_lbl_kv);
     std::swap(hb.name_bytes, o_name_bytes), std::swap(hb.gen_bytes, o_gen_bytes);
-    header_row(nullptr, nullptr, 0, false);
+    header_row(nullptr, nullptr, 0, false, true);
     std::swap(hb.flags, o_flags), std::swap(hb.kind_sid, o_kind), std::swap(hb.group_sid, o_group), std::swap(hb.nsn_off, o_nsn_off), std::swap(hb.nsn_bytes, o_nsn_bytes);
     std::swap(hb.name_off, o_name_off), std::swap(hb.gen_off, o_gen_off), std::swap(hb.lbl_off, o_lbl_off), std::swap(hb.lbl_kv, o_lbl_kv);
     std::swap(hb.name_bytes, o_name_bytes), std::swap(hb.gen_bytes, o_gen_bytes);
@@ -1900,6 +1903,10 @@ std::shared_ptr<HostBatch> Engine::flatten(const ObjIn* objs, size_t n, const Co
     hb.obj_errors.reserve(hb.n);
     for (auto& p : parts) append(hb.obj_errors, p->hb.obj_errors);
     for (auto& p : parts) hb.gvk_lo = std::min(hb.gvk_lo, p->hb.gvk_lo), hb.gvk_hi = std::max(hb.gvk_hi, p->hb.gvk_hi);
+  });
+  tasks.push_back([&]() {
+    hb.gvk.reserve(hb.n);
+    for (auto& p : parts) append(hb.gvk, p->hb.gvk);
   });
   for (size_t s2 = 1; s2 < nscopes; ++s2)
     tasks.push_back([&, s2]() {

@@ -57,6 +57,7 @@ struct HostBatch {
   uint64_t alg_bytes = 0;                      // bytes of every array the kernel may read (each counted once)
   uint64_t schema_version = 0;
   uint64_t gvk_lo = ~0ull, gvk_hi = 0;         // min / max hash of (apiVersion, kind) over the objects that were not skipped
+  std::vector<uint64_t> gvk;                   // [n] that hash per object, 0 for a skipped one (the audit ranks objects by kind)
 };
 
 struct MatchSpec {

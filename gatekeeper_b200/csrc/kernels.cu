@@ -4,6 +4,8 @@
 // gather path, where torch.distributed owns the buffers).
 #include <cuda_runtime.h>
 
+#include <cub/cub.cuh>
+
 #include <algorithm>
 #include <chrono>
 #include <functional>
@@ -16,6 +18,7 @@
 
 #include <list>
 #include <sstream>
+#include <tuple>
 
 #include "backend.hpp"
 #include "ingest_kernels.cuh"
@@ -65,9 +68,160 @@ struct DevBatch {
   uint32_t ntiles = 0, slot_words = 0, tile = 0;
   uint64_t prog_version = 0;
   bool gvk_uniform = false;   // every object that was not skipped has the same apiVersion and kind
+  unsigned long long* gvk = nullptr;   // [n] hash of (apiVersion, kind) per object, 0 for a skipped one (audit_candidates)
   std::vector<uint32_t> cap;  // rows of the largest tile per scope (sizes the slot area of any netlist over this batch)
   bool fork = false;          // a view made by fork_batch: arena and tiling belong to the batch it was forked from
 };
+
+// ---- audit candidates (Backend::audit_candidates): rank the batch's identities, then select per constraint
+// (group, version, kind) arrive as one rank per object (gr, from the page's few distinct apiVersion / kind pairs ranked on the host by
+// their decoded bytes); namespace and name are the decoded bytes of the batch header, read as IdView reads them (audit.cpp).
+struct GkIdLess {
+  const uint32_t* gr;
+  const uint32_t* flags;
+  const uint32_t* ns_off;
+  const uint8_t* ns;
+  const uint32_t* nm_off;
+  const uint8_t* nm;
+  static __device__ int bytes(const uint8_t* a, uint32_t al, const uint8_t* b, uint32_t bl) {
+    const uint32_t m = al < bl ? al : bl;
+    for (uint32_t i = 0; i < m; ++i)
+      if (a[i] != b[i]) return a[i] < b[i] ? -1 : 1;
+    return al < bl ? -1 : al > bl ? 1 : 0;
+  }
+  __device__ uint32_t ns_len(uint32_t o) const {
+    const uint32_t fl = flags[o];
+    return ((fl & GK_F_IS_NS) || !(fl & GK_F_NSNAME)) ? 0u : ns_off[o + 1] - ns_off[o];
+  }
+  __device__ int cmp(uint32_t a, uint32_t b) const {
+    if (gr[a] != gr[b]) return gr[a] < gr[b] ? -1 : 1;
+    const int r = bytes(ns + ns_off[a], ns_len(a), ns + ns_off[b], ns_len(b));
+    return r ? r : bytes(nm + nm_off[a], nm_off[a + 1] - nm_off[a], nm + nm_off[b], nm_off[b + 1] - nm_off[b]);
+  }
+  __device__ bool operator()(uint32_t a, uint32_t b) const { return cmp(a, b) < 0; }
+};
+
+__device__ __forceinline__ uint32_t gk_gvk_slot(unsigned long long k, uint32_t mask) { return (uint32_t)((k * 0x9E3779B97F4A7C15ull) >> 40) & mask; }
+
+// distinct apiVersion / kind hashes of the page into an open-addressing table (keys 0 = empty), with the smallest object of each
+__global__ void gk_gvk_insert_kernel(const unsigned long long* gvk, uint32_t n, unsigned long long* keys, uint32_t* rep, uint32_t mask) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const unsigned long long k = gvk[i];
+    if (!k) continue;
+    for (uint32_t s = gk_gvk_slot(k, mask);; s = (s + 1) & mask) {
+      const unsigned long long prev = atomicCAS(&keys[s], 0ull, k);
+      if (prev == 0ull || prev == k) {
+        atomicMin(&rep[s], i);
+        break;
+      }
+    }
+  }
+}
+__global__ void gk_gvk_collect_kernel(const unsigned long long* keys, const uint32_t* rep, uint32_t cap, uint32_t* cnt, uint32_t* out) {
+  for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < cap; s += gridDim.x * blockDim.x)
+    if (keys[s]) {
+      const uint32_t j = atomicAdd(cnt, 1u);
+      out[2 * j] = s;
+      out[2 * j + 1] = rep[s];
+    }
+}
+// rank of each table entry (slot, rank pairs from the host) into rep, then one rank per object
+__global__ void gk_gvk_assign_kernel(const uint32_t* pairs, uint32_t m, uint32_t* rep) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < m) rep[pairs[2 * j]] = pairs[2 * j + 1];
+}
+__global__ void gk_gvk_map_kernel(const unsigned long long* gvk, uint32_t n, const unsigned long long* keys, const uint32_t* rank, uint32_t mask,
+                                  uint32_t* gr, uint32_t* perm) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const unsigned long long k = gvk[i];
+    uint32_t r = 0;
+    if (k)
+      for (uint32_t s = gk_gvk_slot(k, mask);; s = (s + 1) & mask)
+        if (keys[s] == k) {
+          r = rank[s];
+          break;
+        }
+    gr[i] = r;
+    perm[i] = i;
+  }
+}
+// after the sort: 1 where a sorted position starts a new identity (then scanned into the identity's rank)
+__global__ void gk_id_heads_kernel(const uint32_t* perm, uint32_t n, GkIdLess id, uint32_t* head) {
+  for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) head[p] = p && id.cmp(perm[p - 1], perm[p]) != 0;
+}
+__global__ void gk_id_scatter_kernel(const uint32_t* perm, const uint32_t* grp, uint32_t n, uint32_t* rank) {
+  for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) rank[perm[p]] = grp[p];
+}
+constexpr uint32_t kSelChunk = 1024;   // sorted positions per block of the per-constraint counts
+// cnt[b * C + c]: objects with bit c among the sorted positions [b * kSelChunk, (b + 1) * kSelChunk)
+__global__ void __launch_bounds__(256) gk_sel_count_kernel(const uint32_t* perm, const uint32_t* viol, uint32_t n, uint32_t words, uint32_t C, uint32_t* cnt) {
+  extern __shared__ uint32_t sh[];
+  for (uint32_t c = threadIdx.x; c < C; c += blockDim.x) sh[c] = 0;
+  __syncthreads();
+  const uint32_t lo = blockIdx.x * kSelChunk, hi = min(n, lo + kSelChunk);
+  for (uint32_t p = lo + threadIdx.x; p < hi; p += blockDim.x) {
+    const uint32_t* row = viol + (size_t)perm[p] * words;
+    for (uint32_t w = 0; w < words; ++w)
+      for (uint32_t v = row[w]; v; v &= v - 1) {
+        const uint32_t c = w * 32 + (uint32_t)__ffs(v) - 1;
+        if (c < C) atomicAdd(&sh[c], 1u);
+      }
+  }
+  __syncthreads();
+  for (uint32_t c = threadIdx.x; c < C; c += blockDim.x) cnt[(size_t)blockIdx.x * C + c] = sh[c];
+}
+// one warp per constraint: the sorted position of its limit-th flagged object -> thr[c] = that object's rank (all ones: fewer than limit)
+__global__ void gk_sel_thresh_kernel(const uint32_t* perm, const uint32_t* viol, const uint32_t* cnt, const uint32_t* rank, uint32_t n, uint32_t words,
+                                     uint32_t C, uint32_t nb, uint32_t limit, uint32_t* thr) {
+  const uint32_t c = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x & 31u;
+  if (c >= C) return;
+  uint32_t acc = 0, need = 0, blk = ~0u;
+  for (uint32_t base = 0; base < nb && blk == ~0u; base += 32) {
+    const uint32_t v = base + lane < nb ? cnt[(size_t)(base + lane) * C + c] : 0u;
+    uint32_t s = v;
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xffffffffu, s, d);
+      if (lane >= d) s += t;
+    }
+    const uint32_t hit = __ballot_sync(0xffffffffu, acc + s >= limit);
+    if (hit) {
+      const uint32_t f = (uint32_t)__ffs(hit) - 1;
+      need = limit - (acc + __shfl_sync(0xffffffffu, s - v, f));   // 1-based among the block's flagged positions
+      blk = base + f;
+    }
+    acc += __shfl_sync(0xffffffffu, s, 31);
+  }
+  if (blk == ~0u) {
+    if (!lane) thr[c] = ~0u;
+    return;
+  }
+  const uint32_t lo = blk * kSelChunk, hi = min(n, lo + kSelChunk);
+  for (uint32_t p = lo; p < hi; p += 32) {
+    const uint32_t q = p + lane;
+    const bool b = q < hi && (viol[(size_t)perm[q] * words + (c >> 5)] >> (c & 31u) & 1u);
+    const uint32_t bal = __ballot_sync(0xffffffffu, b);
+    const uint32_t k = (uint32_t)__popc(bal);
+    if (need <= k) {
+      uint32_t m = bal;
+      for (uint32_t j = 1; j < need; ++j) m &= m - 1;
+      if (!lane) thr[c] = rank[perm[p + (uint32_t)__ffs(m) - 1]];
+      return;
+    }
+    need -= k;
+  }
+}
+__global__ void gk_sel_emit_kernel(const uint32_t* viol, const uint32_t* rank, const uint32_t* thr, uint32_t n, uint32_t words, uint32_t C, uint32_t* cand) {
+  const size_t total = (size_t)n * words;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const uint32_t o = (uint32_t)(i / words), w = (uint32_t)(i % words), r = rank[o];
+    uint32_t out = 0;
+    for (uint32_t v = viol[i]; v; v &= v - 1) {
+      const uint32_t k = (uint32_t)__ffs(v) - 1, c = w * 32 + k;
+      if (c < C && r <= thr[c]) out |= 1u << k;
+    }
+    cand[i] = out;
+  }
+}
 
 class CudaBackend : public Backend {
  public:
@@ -229,6 +383,7 @@ class CudaBackend : public Backend {
     db->gvk_uniform = hb.gvk_hi == 0 || hb.gvk_lo == hb.gvk_hi;
     dmalloc(&db->arena, db->bytes);
     dmalloc(&db->d_tile_lo, tile_lo.size() * 4 + 64);
+    if (hb.n) dmalloc(&db->gvk, (size_t)hb.n * 8);
     finish_batch(db, c, cap);
     const size_t tables_bytes = c.ops.size() * sizeof(GkOp) + c.pool.size() * 4 + c.outs.size() * sizeof(GkOutEnt);
     cudaEvent_t a, b;
@@ -249,6 +404,7 @@ class CudaBackend : public Backend {
       CK(cudaEventRecord(a, stream_));
       CK(cudaMemcpyAsync(db->arena, image, plan.total, cudaMemcpyHostToDevice, stream_));
       CK(cudaMemcpyAsync(db->d_tile_lo, tile_lo.data(), tile_lo.size() * 4, cudaMemcpyHostToDevice, stream_));
+      if (hb.n) CK(cudaMemcpyAsync(db->gvk, hb.gvk.data(), (size_t)hb.n * 8, cudaMemcpyHostToDevice, stream_));
       CK(cudaEventRecord(b, stream_));
       CK(cudaStreamSynchronize(stream_));
     }
@@ -379,6 +535,7 @@ class CudaBackend : public Backend {
     dfree(db->viol);
     dfree(db->err);
     if (!db->fork) dfree(db->d_tile_lo);
+    if (!db->fork) dfree(db->gvk);
     dfree(db->d_tile_list);
     dfree(db->d_ops);
     dfree(db->d_pool);
@@ -1100,7 +1257,8 @@ class CudaBackend : public Backend {
     {
       const unsigned long long init[2] = {~0ull, 0ull};
       push_small(d_mm, init, 16);
-      out.gvk = n ? reinterpret_cast<unsigned long long*>(talloc((size_t)n * 8)) : nullptr;
+      if (n) dmalloc(&db->gvk, (size_t)n * 8);
+      out.gvk = db->gvk;
     }
     if (!n) CK(cudaMemsetAsync(A, 0, db->bytes, stream_));   // (no kernel writes the closing CSR entries of an empty batch)
     // the CSR offsets of the scopes and of the byte columns are the scanned counts of the count phase
@@ -1272,6 +1430,7 @@ class CudaBackend : public Backend {
     f->ntiles = db->ntiles;
     f->tile = db->tile;
     f->gvk_uniform = db->gvk_uniform;
+    f->gvk = db->gvk;
     f->fork = true;
     f->prog_version = other.version;
     std::unique_ptr<DevBatch, std::function<void(DevBatch*)>> guard(f, [this](DevBatch* x) { release(x); });
@@ -1302,6 +1461,121 @@ class CudaBackend : public Backend {
     if (!out.ns_bytes.empty()) CK(cudaMemcpyAsync(out.ns_bytes.data(), db->hdr.nsn_bytes, out.ns_bytes.size(), cudaMemcpyDeviceToHost, stream_));
     if (!out.name_bytes.empty()) CK(cudaMemcpyAsync(out.name_bytes.data(), db->hdr.name_bytes, out.name_bytes.size(), cudaMemcpyDeviceToHost, stream_));
     CK(cudaStreamSynchronize(stream_));
+  }
+
+  // Ranking: the page's distinct apiVersion / kind hashes (a device hash table) are decoded on the host from one object each and ranked
+  // by (group, version, kind); every object gets its triple's rank; the objects are merge-sorted by (that rank, namespace, name) and the
+  // heads of equal runs scanned into one rank per identity.  Selection: per block of sorted positions and per constraint, the count of
+  // flagged objects; per constraint (one warp), the rank of its limit-th flagged object; then every flagged bit at or below it.
+  void audit_candidates(void* b, const uint32_t* viol, uint32_t words, uint32_t C, uint32_t limit, const GvkOf& gvk_of, std::vector<uint32_t>& cand,
+                        float* device_ms) override {
+    auto* db = static_cast<DevBatch*>(b);
+    std::lock_guard<std::mutex> l(mu_);
+    CK(cudaSetDevice(device_));
+    const uint32_t n = db->n;
+    cand.assign((size_t)n * words, 0u);
+    if (device_ms) *device_ms = 0.f;
+    if (!n || !C || !words) return;
+    if (!db->gvk) throw BackendError{"audit candidates: the batch holds no apiVersion / kind hashes"};
+    std::vector<void*> temps;
+    struct Free {
+      CudaBackend* be;
+      std::vector<void*>& t;
+      ~Free() {
+        for (void* p : t) be->dfree(p);
+      }
+    } free_temps{this, temps};
+    auto take = [&](size_t bytes) {
+      void* p = nullptr;
+      dmalloc(&p, bytes);
+      temps.push_back(p);
+      return p;
+    };
+    uint32_t cap = 1024;
+    while (cap < 2 * n) cap <<= 1;
+    const uint32_t mask = cap - 1, T = 256, grid = std::min<uint32_t>((n + T - 1) / T, (uint32_t)sms_ * 16);
+    auto* keys = static_cast<unsigned long long*>(take((size_t)cap * 8));
+    auto* rep = static_cast<uint32_t*>(take((size_t)cap * 4));
+    auto* d_cnt = static_cast<uint32_t*>(take(64));
+    auto* d_list = static_cast<uint32_t*>(take((size_t)2 * n * 4));
+    auto* d_viol = static_cast<uint32_t*>(take((size_t)n * words * 4));
+    cudaEvent_t e0, e1, e2, e3;
+    for (cudaEvent_t* e : {&e0, &e1, &e2, &e3}) CK(cudaEventCreate(e));
+    struct Ev {
+      cudaEvent_t* e[4];
+      ~Ev() {
+        for (auto x : e) cudaEventDestroy(*x);
+      }
+    } ev_guard{{&e0, &e1, &e2, &e3}};
+    CK(cudaMemcpyAsync(d_viol, viol, (size_t)n * words * 4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaEventRecord(e0, stream_));
+    CK(cudaMemsetAsync(keys, 0, (size_t)cap * 8, stream_));
+    CK(cudaMemsetAsync(rep, 0xff, (size_t)cap * 4, stream_));
+    CK(cudaMemsetAsync(d_cnt, 0, 4, stream_));
+    gk_gvk_insert_kernel<<<grid, T, 0, stream_>>>(db->gvk, n, keys, rep, mask);
+    gk_gvk_collect_kernel<<<std::min<uint32_t>((cap + T - 1) / T, (uint32_t)sms_ * 16), T, 0, stream_>>>(keys, rep, cap, d_cnt, d_list);
+    CK(cudaEventRecord(e1, stream_));
+    uint32_t m = 0;
+    CK(cudaMemcpyAsync(&m, d_cnt, 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
+    std::vector<uint32_t> list((size_t)2 * m);
+    if (m) CK(cudaMemcpy(list.data(), d_list, list.size() * 4, cudaMemcpyDeviceToHost));
+    // (group, version, kind) of one object per distinct hash, ranked; equal triples (differently escaped JSON) share a rank
+    struct Gvk {
+      std::string g, v, k;
+      uint32_t j;
+    };
+    std::vector<Gvk> tri(m);
+    for (uint32_t j = 0; j < m; ++j) {
+      tri[j].j = j;
+      gvk_of(list[2 * j + 1], tri[j].g, tri[j].v, tri[j].k);
+    }
+    auto key = [](const Gvk& x) { return std::tie(x.g, x.v, x.k); };
+    std::sort(tri.begin(), tri.end(), [&](const Gvk& a, const Gvk& c2) { return key(a) < key(c2); });
+    std::vector<uint32_t> pairs((size_t)2 * m);
+    for (uint32_t r = 0, i = 0; i < m; ++i) {
+      if (i && key(tri[i - 1]) != key(tri[i])) ++r;
+      pairs[2 * i] = list[2 * tri[i].j];
+      pairs[2 * i + 1] = r;
+    }
+    auto* gr = static_cast<uint32_t*>(take((size_t)n * 4));
+    auto* perm = static_cast<uint32_t*>(take((size_t)n * 4));
+    auto* head = static_cast<uint32_t*>(take((size_t)n * 4));
+    auto* rank = static_cast<uint32_t*>(take((size_t)n * 4));
+    CK(cudaEventRecord(e2, stream_));
+    if (m) {
+      CK(cudaMemcpyAsync(d_list, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, stream_));
+      gk_gvk_assign_kernel<<<(m + T - 1) / T, T, 0, stream_>>>(d_list, m, rep);
+    }
+    gk_gvk_map_kernel<<<grid, T, 0, stream_>>>(db->gvk, n, keys, rep, mask, gr, perm);
+    const GkIdLess less{gr, db->hdr.flags, db->hdr.nsn_off, db->hdr.nsn_bytes, db->hdr.name_off, db->hdr.name_bytes};
+    size_t sort_bytes = 0, scan_bytes = 0;
+    CK(cub::DeviceMergeSort::SortKeys(nullptr, sort_bytes, perm, (int64_t)n, less, stream_));
+    CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, head, rank, (int64_t)n, stream_));
+    void* cub_tmp = take(std::max(sort_bytes, scan_bytes));
+    CK(cub::DeviceMergeSort::SortKeys(cub_tmp, sort_bytes, perm, (int64_t)n, less, stream_));
+    gk_id_heads_kernel<<<grid, T, 0, stream_>>>(perm, n, less, head);
+    CK(cub::DeviceScan::InclusiveSum(cub_tmp, scan_bytes, head, gr, (int64_t)n, stream_));   // (gr is free again: the sort is done)
+    gk_id_scatter_kernel<<<grid, T, 0, stream_>>>(perm, gr, n, rank);
+    const uint32_t nb = (n + kSelChunk - 1) / kSelChunk;
+    auto* cnt = static_cast<uint32_t*>(take((size_t)nb * C * 4));
+    auto* thr = static_cast<uint32_t*>(take((size_t)C * 4));
+    auto* d_cand = static_cast<uint32_t*>(take((size_t)n * words * 4));
+    if ((size_t)C * 4 > max_smem_) throw BackendError{"audit candidates: too many constraints for one block's counters"};
+    if ((size_t)C * 4 > 48 * 1024) CK(cudaFuncSetAttribute(gk_sel_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(C * 4)));
+    gk_sel_count_kernel<<<nb, 256, (size_t)C * 4, stream_>>>(perm, d_viol, n, words, C, cnt);
+    gk_sel_thresh_kernel<<<(C * 32 + 255) / 256, 256, 0, stream_>>>(perm, d_viol, cnt, rank, n, words, C, nb, limit, thr);
+    gk_sel_emit_kernel<<<std::min<uint32_t>((uint32_t)(((size_t)n * words + T - 1) / T), (uint32_t)sms_ * 16), T, 0, stream_>>>(d_viol, rank, thr, n, words, C, d_cand);
+    CK(cudaEventRecord(e3, stream_));
+    CK(cudaMemcpyAsync(cand.data(), d_cand, (size_t)n * words * 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
+    launches_ += 8 + (m ? 1 : 0);
+    float a = 0.f, c2 = 0.f;
+    cudaEventElapsedTime(&a, e0, e1);
+    cudaEventElapsedTime(&c2, e2, e3);
+    if (device_ms) *device_ms = a + c2;
   }
 
   // ---- front buffers: a page's JSON, offsets and tape.  Two of them, so that page k+1 streams in (copy stream + front stream)

@@ -71,7 +71,7 @@ EXPORTS = [
     "gk_batch_eval_device_peers", "gk_batch_upload_blob", "gk_review_blob", "gk_set_excluded_namespaces", "gk_audit_begin", "gk_audit_add_batch", "gk_audit_report",
     "gk_audit_end", "gk_validation_messages", "gk_host_cpus", "gk_pin_host", "gk_blob_prefetch", "gk_coalescer_create", "gk_coalescer_review", "gk_coalescer_stats",
     "gk_coalescer_destroy", "gk_batch_size", "gk_batch_alg_bytes", "gk_batch_free", "gk_batch_refresh", "gk_free_result", "gk_free_str", "gk_dump",
-    "gk_stat_description",
+    "gk_stat_description", "gk_audit_add_batch_ordered", "gk_audit_select_ms", "gk_audit_export", "gk_audit_merge",
 ]
 
 
@@ -121,6 +121,11 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.gk_audit_begin.argtypes = [P, U32, U32, PP]
     lib.gk_audit_begin.restype = P
     lib.gk_audit_add_batch.argtypes = [P, P, S, PP]
+    lib.gk_audit_add_batch_ordered.argtypes = [P, P, S, PP]
+    lib.gk_audit_select_ms.argtypes = [P]
+    lib.gk_audit_select_ms.restype = C.c_float
+    lib.gk_audit_export.argtypes = [P, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), PP]
+    lib.gk_audit_merge.argtypes = [P, C.c_char_p, C.c_size_t, PP]
     lib.gk_audit_report.argtypes = [P, PP]
     lib.gk_audit_report.restype = C.c_void_p
     lib.gk_audit_end.argtypes = [P]
@@ -589,6 +594,29 @@ class AuditRun:
     def add_batch(self, rb: "ResidentBatch", enforcement_point: str = AUDIT_EP):
         err = C.c_char_p()
         self.drv._check(self.drv._lib.gk_audit_add_batch(self._a, rb.h, enforcement_point.encode(), C.byref(err)), err)
+
+    def add_batch_ordered(self, rb: "ResidentBatch", enforcement_point: str = AUDIT_EP):
+        """add_batch with the candidates ranked and selected on the device: the lazy path for a page of any mix of kinds."""
+        err = C.c_char_p()
+        self.drv._check(self.drv._lib.gk_audit_add_batch_ordered(self._a, rb.h, enforcement_point.encode(), C.byref(err)), err)
+
+    def select_ms(self) -> float:
+        """Device time of the last add_batch_ordered's ranking and selection kernels (ms)."""
+        return float(self.drv._lib.gk_audit_select_ms(self._a))
+
+    def export(self) -> bytes:
+        """The run's partial state as an opaque, versioned byte string (merge() it into another run)."""
+        err, buf, n = C.c_char_p(), C.c_void_p(), C.c_size_t()
+        self.drv._check(self.drv._lib.gk_audit_export(self._a, C.byref(buf), C.byref(n), C.byref(err)), err)
+        try:
+            return C.string_at(buf, n.value)
+        finally:
+            self.drv._lib.gk_free_str(buf)
+
+    def merge(self, data: bytes):
+        """Fold an exported run in, as if its objects came after this run's."""
+        err = C.c_char_p()
+        self.drv._check(self.drv._lib.gk_audit_merge(self._a, bytes(data), len(data), C.byref(err)), err)
 
     def report(self) -> dict:
         err = C.c_char_p()

@@ -113,3 +113,59 @@ class ShardedSweep:
     def step(self, enforcement_point: str):
         self.evaluate(enforcement_point)
         return self.exchange()
+
+
+class ShardedAudit:
+    """The audit's constraint status over a sharded sweep: every rank folds its own pages into an AuditRun
+    (add_batch_ordered: the lazy path for any mix of kinds), then the runs' exports are all-gathered and merged in rank
+    order, so that every rank holds the report one run over all shards in rank order would give.
+
+    The exchange is two collectives on the default group (gloo or NCCL): the export sizes, then the exports padded to the
+    largest as uint8 tensors."""
+
+    def __init__(self, drv, violations_limit: int = 0, msg_size: int = 0, device=None):
+        from gatekeeper_b200 import driver as D
+        self.drv, self.limit, self.msg_size = drv, violations_limit, msg_size
+        self.run = D.AuditRun(drv, violations_limit, msg_size)
+        self.device = device
+        self.merged = None
+        self.timing = {}
+
+    def add_batch(self, rb, enforcement_point: str):
+        self.run.add_batch_ordered(rb, enforcement_point)
+
+    def exchange(self) -> dict:
+        """All-gather every rank's run, merge them in rank order; returns the merged report (the same on every rank)."""
+        import time
+        import torch
+        import torch.distributed as dist
+        from gatekeeper_b200 import driver as D
+        dev = self.device if self.device is not None else torch.device("cpu")
+        world = dist.get_world_size() if dist.is_initialized() else 1
+        t0 = time.perf_counter()
+        mine = self.run.export()
+        t1 = time.perf_counter()
+        if world == 1:
+            parts = [mine]
+        else:
+            size = torch.tensor([len(mine)], dtype=torch.int64, device=dev)
+            sizes = [torch.zeros(1, dtype=torch.int64, device=dev) for _ in range(world)]
+            dist.all_gather(sizes, size)
+            lens = [int(s.item()) for s in sizes]
+            pad = max(lens)
+            send = torch.zeros(pad, dtype=torch.uint8)
+            send[:len(mine)] = torch.frombuffer(bytearray(mine), dtype=torch.uint8)
+            send = send.to(dev)
+            recv = [torch.zeros(pad, dtype=torch.uint8, device=dev) for _ in range(world)]
+            dist.all_gather(recv, send)
+            parts = [bytes(r[:k].cpu().numpy().tobytes()) for r, k in zip(recv, lens)]
+        t2 = time.perf_counter()
+        merged = D.AuditRun(self.drv, self.limit, self.msg_size)
+        for p in parts:
+            merged.merge(p)
+        t3 = time.perf_counter()
+        if self.merged is not None:
+            self.merged.close()
+        self.merged = merged
+        self.timing = {"export_ms": (t1 - t0) * 1e3, "exchange_ms": (t2 - t1) * 1e3, "merge_ms": (t3 - t2) * 1e3, "bytes": sum(len(p) for p in parts)}
+        return merged.report()

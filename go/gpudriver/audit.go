@@ -85,6 +85,46 @@ func (r *AuditRun) AddPage(b *C.gk_batch_t, enforcementPoint string) error {
 	return nil
 }
 
+// AddPageOrdered is AddPage with the candidates ranked and selected on the GPU (gk_audit_add_batch_ordered): pages of any mix of
+// kinds take the lazy path.  The report equals AddPage's except for pairsEvaluated / pairsCounted.
+func (r *AuditRun) AddPageOrdered(b *C.gk_batch_t, enforcementPoint string) error {
+	cep := C.CString(enforcementPoint)
+	defer C.free(unsafe.Pointer(cep))
+	var cerr *C.char
+	if rc := C.gk_audit_add_batch_ordered(r.a, b, cep, &cerr); rc != 0 {
+		return takeErr(cerr)
+	}
+	return nil
+}
+
+// Export returns the run's partial state as an opaque versioned byte string (gk_audit_export), for Merge on another process.
+func (r *AuditRun) Export() ([]byte, error) {
+	var buf *C.char
+	var n C.size_t
+	var cerr *C.char
+	if rc := C.gk_audit_export(r.a, &buf, &n, &cerr); rc != 0 {
+		return nil, takeErr(cerr)
+	}
+	defer C.gk_free_str(buf)
+	return C.GoBytes(unsafe.Pointer(buf), C.int(n)), nil
+}
+
+// Merge folds an exported run in as if its objects came after this run's (gk_audit_merge): merging the shards' exports in shard
+// order reports what one run over all shards would.  A damaged export, another format version or another limit / msgSize is
+// refused and leaves the run unchanged.
+func (r *AuditRun) Merge(data []byte) error {
+	var cerr *C.char
+	var p *C.char
+	if len(data) > 0 {
+		p = (*C.char)(C.CBytes(data))
+		defer C.free(unsafe.Pointer(p))
+	}
+	if rc := C.gk_audit_merge(r.a, p, C.size_t(len(data)), &cerr); rc != 0 {
+		return takeErr(cerr)
+	}
+	return nil
+}
+
 // RefreshBatch brings a resident batch to the current constraint set, excluder patterns and data.inventory (gk_batch_refresh), so
 // that an audit run can add it again after a template or constraint changed.  A page uploaded with GK_F_KEEP_SOURCE is re-extracted
 // from its token tape in HBM; any other is flattened again from the objects or blob it was uploaded from, which must still be alive.

@@ -210,6 +210,22 @@ gk_audit_t* gk_audit_begin(gk_engine_t* e, uint32_t violations_limit, uint32_t m
 /* evaluate a resident batch at the enforcement point and fold every result into the run (messages are rendered for the
  * flagged pairs on all host cores) */
 int gk_audit_add_batch(gk_audit_t* a, gk_batch_t* b, const char* enforcement_point, char** err);
+/* gk_audit_add_batch with the candidates selected on the device, for a page of any mix of kinds (manager.go:886-945; the order is
+ * SVQueue.Less, manager.go:117-137): the batch's objects are ranked by (group, version, kind, namespace, name) and, per constraint,
+ * only the flagged objects at or below the `violations_limit`-th smallest identity (ties included) are rendered on the host; the
+ * other pairs of constraints with one result per pair are counted from the bitmap.  The ambiguity netlist runs whatever the kinds.
+ * The report equals gk_audit_add_batch's except for "pairsEvaluated" / "pairsCounted". */
+int gk_audit_add_batch_ordered(gk_audit_t* a, gk_batch_t* b, const char* enforcement_point, char** err);
+/* device time (ms) of the ranking and selection of the last gk_audit_add_batch_ordered */
+float gk_audit_select_ms(gk_audit_t* a);
+/* A sharded sweep (manager.go:886-945 over each shard, one updateConstraintStatus at the end: manager.go:984-1041).
+ * gk_audit_export: the run's partial state -- per-constraint totals and status lists, per-action totals, object / result / pair
+ * counters, object errors -- as an opaque versioned byte string in *buf (free with gk_free_str), *len bytes.
+ * gk_audit_merge: folds an exported run into `a` as if its objects came after a's (object-error indices are offset by the objects
+ * `a` has seen): merging the shards' exports in shard order reports what one run over all shards in that order would.  A truncated
+ * or corrupted buffer, another format version, or another violations_limit / msg_size: GK_ERR_INVALID, and `a` is unchanged. */
+int gk_audit_export(gk_audit_t* a, char** buf, size_t* len, char** err);
+int gk_audit_merge(gk_audit_t* a, const char* buf, size_t len, char** err);
 /* JSON: {"objects", "results", "totalViolations": {"Kind/name": n}, "totalViolationsPerEnforcementAction": {action: n},
  * "violations": {"Kind/name": [StatusViolation...]}} -- lists in the order updateConstraintStatus emits them (descending).
  * Caller frees with gk_free_str. */
