@@ -750,8 +750,8 @@ class CudaBackend : public Backend {
     }
     se.compile_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     if (getenv("GK_TRACE_LAUNCH"))
-      fprintf(stderr, "[spec] constraint set %llu: %zu bytes of source, %zu atoms as immediates / %zu generic, NVRTC %.0f ms, state %d\n", (unsigned long long)se.version,
-              se.src.src.size(), se.src.n_fast, se.src.n_generic, se.compile_ms, se.state);
+      fprintf(stderr, "[spec] constraint set %llu: %zu bytes of source, %zu atoms as immediates / %zu generic, NVRTC %.0f ms, state %d; %s\n", (unsigned long long)se.version,
+              se.src.src.size(), se.src.n_fast, se.src.n_generic, se.compile_ms, se.state, se.src.fold_text().c_str());
   }
 
   void eval(void* b, const std::vector<uint32_t>& active, EvalOut& out, bool copy_back) override {
@@ -1748,7 +1748,7 @@ class CudaBackend : public Backend {
   // 256 threads walk a 512-object tile (two objects each), at least two CTAs per SM (<= 128 registers) so that one CTA's staging
   // overlaps another's object walk: the fastest of 512 x 1, 256 x 2 and 256 x 3 over configs 2, 4 and 5 (256 x 3 spills at config 2)
   int spec_threads_ = getenv("GK_SPEC_THREADS") ? std::min(1024, std::max(32, atoi(getenv("GK_SPEC_THREADS")) / 32 * 32)) : 256;
-  int spec_minb_ = getenv("GK_SPEC_MINB") ? std::max(1, atoi(getenv("GK_SPEC_MINB"))) : 2;
+  int spec_minb_ = getenv("GK_SPEC_MINB") ? std::max(1, atoi(getenv("GK_SPEC_MINB"))) : 3;   // 256 x 3: an 80-register cap, measured best or level at configs 2, 4 and 5 (DESIGN 5a)
   const char* last_kernel_ = "gk_eval_kernel";
   bool spec_next_ = false;
   size_t spec_smem_ = 0;      // dynamic shared memory of the next launch of the generated kernel (set with spec_next_)

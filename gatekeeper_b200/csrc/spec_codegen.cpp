@@ -62,7 +62,7 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
   uint32_t* s_tot = act + GK_SPEC_W * 32u;
   uint32_t* s_err = s_tot + GK_SPEC_W * 32u;
   uint32_t* actw = s_err + GK_SPEC_W * 32u;   // the enforcement-point mask packed: bit c of word c / 32
-  uint32_t* stg = reinterpret_cast<uint32_t*>(smem + GK_SPEC_STAGE_AT);   // the tile's staged atom bits and offsets (gk_spec_stage)
+  uint32_t* stg = reinterpret_cast<uint32_t*>(smem + GK_SPEC_STAGE_AT);   // the tile's staged export bits and offsets (gk_spec_stage)
   {
     const uint4* a = reinterpret_cast<const uint4*>(p.batch.cols);
     uint4* d = reinterpret_cast<uint4*>(cols);
@@ -387,6 +387,11 @@ struct SpecNode {
   std::string code;
   std::vector<uint32_t> deps;
   bool done = false;
+  // what the row-local classification (spec_codegen()) reads: the op's kind and scope; of a gate its inputs (variable, or -1 for a
+  // slot never written = 0; negated?) and flags, so that phase 1 can write it as a boolean expression; of a constant its value
+  uint32_t kind = GK_N_END, level = 0;
+  std::vector<std::pair<int, bool>> in;
+  bool is_or = false, neg_out = false, one = false;
 };
 
 struct Gen {
@@ -435,11 +440,12 @@ struct Gen {
     return nvar++;
   }
   uint32_t fresh(uint32_t slot) { return fresh(slot, (int)nodes.size()); }   // defined by the node being built
+  SpecNode cur_node;                       // (its structured part, filled in by op())
   void finish_node() {
-    SpecNode n;
-    n.code = body.str();
-    n.deps = deps;
-    nodes.push_back(std::move(n));
+    cur_node.code = body.str();
+    cur_node.deps = deps;
+    nodes.push_back(std::move(cur_node));
+    cur_node = SpecNode();
     body.str("");
     deps.clear();
   }
@@ -531,6 +537,8 @@ struct Gen {
   void op(const GkOp& op) {
     const uint32_t kind = op.w0 & 0xffu, level = (op.w0 >> 8) & 0xffu, out = op.w0 >> 16;
     const std::string L = std::to_string(level);
+    cur_node.kind = kind;
+    cur_node.level = level;
     switch (kind) {
       case GK_N_ATOM: atom(level, out, op.w1 >> 8, op.w1 & 0xffu, op.w2, op.w3); break;
       case GK_N_ATOMS:
@@ -542,6 +550,7 @@ struct Gen {
       case GK_N_CONST: {
         use_scope(level);
         const uint32_t v = fresh(out);
+        cur_node.one = (op.w1 & 1u) != 0u;
         body << "  const uint32_t v" << v << " = " << ((op.w1 & 1u) ? "f" + L : std::string("0u")) << ";\n";
         break;
       }
@@ -554,8 +563,12 @@ struct Gen {
           const uint32_t in = c.pool[op.w1 + j];
           const bool neg = (in >> 31) != 0u;
           any_neg = any_neg || neg;
-          e += (j ? (is_or ? " | " : " & ") : "") + std::string(neg ? "~" : "") + rd(in & 0xffffu);
+          const uint32_t slot = in & 0xffffu;
+          cur_node.in.emplace_back(slot < cur.size() ? cur[slot] : -1, neg);
+          e += (j ? (is_or ? " | " : " & ") : "") + std::string(neg ? "~" : "") + rd(slot);
         }
+        cur_node.is_or = is_or;
+        cur_node.neg_out = neg_out;
         if (op.w3 == 0) e = is_or ? "0u" : "0xffffffffu", any_neg = true;
         if (neg_out) e = "~(" + e + ")";
         if (any_neg) e = "(" + e + ") & f" + L;
@@ -635,7 +648,7 @@ SpecSource spec_codegen(const Compiled& c) {
   std::ostringstream o;
   o << "// generated by spec_codegen.cpp for constraint-set version " << c.version << ": " << C << " constraints, " << c.ops.size() << " netlist ops\n";
   o << "#define GK_SPEC_C " << C << "u\n#define GK_SPEC_W " << W << "\n";
-  o << "#ifndef GK_SPEC_THREADS\n#define GK_SPEC_THREADS 256\n#endif\n#ifndef GK_SPEC_MINB\n#define GK_SPEC_MINB 2\n#endif\n";
+  o << "#ifndef GK_SPEC_THREADS\n#define GK_SPEC_THREADS 256\n#endif\n#ifndef GK_SPEC_MINB\n#define GK_SPEC_MINB 3\n#endif\n";
   o << "#ifndef GK_SPEC_HOST\n#define GK_LD(p) __ldg(p)   /* pool, cbytes and every batch array are global and read-only here */\n#endif\n";
   o << strip_includes(kSpecHdrProgram) << strip_includes(kSpecHdrVmCore);
   o << R"GKSRC(
@@ -726,9 +739,8 @@ struct uint4 { uint32_t x, y, z, w; };
     order.push_back(std::move(e));
   }
   std::sort(order.begin(), order.end());
-  // ---- atom groups: ONE row loop per scope computes every atom of that scope (~45 mask registers of the container scope alive at
-  // once, some spilled).  A loop per (scope, template kind) keeps fewer masks alive and measured no better: every extra loop is one
-  // more exposed memory latency per object.
+  // ---- atom groups: ONE row loop per scope computes every atom of that scope.  A loop per (scope, template kind) measured no
+  // better: every extra loop is one more exposed memory latency per object.
   std::map<uint32_t, int> group_ix;   // scope -> row loop
   std::vector<std::vector<uint32_t>> groups;
   for (const Ord& e : order) {
@@ -746,19 +758,97 @@ struct uint4 { uint32_t x, y, z, w; };
       groups[(size_t)r.group].push_back(ai);
     }
   }
-  // ---- phase 1, gk_spec_stage(): once per tile the whole CTA evaluates the atoms of every row loop on every row of the tile in that
-  // scope -- consecutive rows in consecutive threads, so the column loads are coalesced and independent -- and stores them as packed
-  // bits in shared memory (ceil(atoms / 32) words per row; bit k of word k / 32 = the loop's k-th atom), together with the tile's
-  // slice of every used nested scope's CSR offsets (tile-relative).  The per-tile layout follows from the rows of every scope in the
+  auto parent_of = [&](uint32_t s) { return (uint32_t)c.schema.scopes[s].parent; };
+  // ---- row-local values and exports.  A variable of scope L is ROW-LOCAL when it is a function of one row of L alone: an atom of L,
+  // or a gate of L whose inputs are row-local values and constants (and at least one of the former).  Phase 1 has every atom of a
+  // row in a register, so it evaluates those gates there and stages only the EXPORTS: the row-local values that something else
+  // reads -- an EXISTS, a broadcast, a gate with an input that is not row-local, a constraint's result.  An export that only
+  // object-level EXISTS read is in ANY form (phase 2 ORs the rows' staged words and tests one bit); every other export is in MASK
+  // form (phase 2 rebuilds the per-row mask, as it did for every atom before).  Constants, and gates of nothing but constants,
+  // are literals in phase 1 and stay the nodes they were in phase 2.
+  enum : uint8_t { kNotExported = 0, kAny = 1, kMask = 2 };
+  std::vector<int> local(g.nvar, -1);      // variable -> the scope it is row-local in
+  std::vector<int8_t> konst(g.nvar, -1);   // variable -> its value in a row that exists, when it is a constant
+  for (uint32_t v = 0; v < g.nvar; ++v) {
+    if (g.atom_of[v] >= 0) {
+      local[v] = (int)g.atoms[(size_t)g.atom_of[v]].scope;
+      continue;
+    }
+    if (g.producer[v] < 0) continue;
+    const SpecNode& n = g.nodes[(size_t)g.producer[v]];
+    if (n.kind == GK_N_CONST) konst[v] = n.one ? 1 : 0;
+    if (n.kind != GK_N_GATE) continue;
+    bool all = true, some = false, val = !n.is_or;
+    for (const auto& in : n.in) {
+      const bool k = in.first < 0 || konst[(size_t)in.first] >= 0, l = !k && local[(size_t)in.first] == (int)n.level;
+      all = all && (k || l);
+      some = some || l;
+      if (k) {
+        const bool x = (in.first >= 0 && konst[(size_t)in.first] == 1) != in.second;
+        val = n.is_or ? (val || x) : (val && x);
+      }
+    }
+    if (all && some) local[v] = (int)n.level;
+    else if (all) konst[v] = (val != n.neg_out) ? 1 : 0;
+  }
+  auto folded = [&](uint32_t v) { return local[v] >= 0 && g.atom_of[v] < 0; };   // a gate phase 1 evaluates
+  std::vector<uint8_t> form(g.nvar, kNotExported), live(g.nvar, 0);
+  {
+    std::vector<uint32_t> todo;
+    auto reach = [&](uint32_t v) {
+      if (!live[v]) live[v] = 1, todo.push_back(v);
+    };
+    for (uint32_t cix = 0; cix < C; ++cix) {
+      const GkOutEnt& oe = c.outs[cix];
+      for (int v : {(oe.flags & 3u) ? -1 : var_of(oe.prog_slot), var_of(oe.match_slot), var_of(oe.err_slot)}) {
+        if (v < 0) continue;
+        reach((uint32_t)v);
+        if (local[(size_t)v] >= 0) form[(size_t)v] = kMask;
+      }
+    }
+    while (!todo.empty()) {
+      const uint32_t v = todo.back();
+      todo.pop_back();
+      if (g.producer[v] < 0) continue;
+      const SpecNode& n = g.nodes[(size_t)g.producer[v]];
+      // (GK_N_ACC2 exists only in the audit's ambiguity netlist, which is interpreted; the generator is handed the decision netlist.
+      // Were one to reach it, its input would be exported in mask form, which the count needs.)
+      const bool any = n.kind == GK_N_ACC && parent_of(n.level) == 0u;
+      for (uint32_t d : n.deps) {
+        reach(d);
+        if (local[d] >= 0 && !folded(v)) form[d] = std::max<uint8_t>(form[d], any ? kAny : kMask);
+      }
+    }
+  }
+  // per row loop: its exports (any form first), and the gates phase 1 evaluates for them, in netlist order
+  std::vector<std::vector<uint32_t>> exports(groups.size()), gates(groups.size());
+  std::vector<uint32_t> nany(groups.size(), 0);
+  std::vector<int> bit_of(g.nvar, -1);     // export -> its bit in the row's staged words
+  for (uint8_t f : {kAny, kMask})
+    for (uint32_t v = 0; v < g.nvar; ++v) {
+      if (!live[v] || form[v] != f) continue;
+      const size_t gi = (size_t)group_ix.at((uint32_t)local[v]);
+      bit_of[v] = (int)exports[gi].size();
+      exports[gi].push_back(v);
+      if (f == kAny) ++nany[gi];
+    }
+  for (uint32_t v = 0; v < g.nvar; ++v)
+    if (live[v] && folded(v)) gates[(size_t)group_ix.at((uint32_t)local[v])].push_back(v);
+  // ---- phase 1, gk_spec_stage(): once per tile the whole CTA evaluates the atoms and the row-local gates of every row loop on every
+  // row of the tile in that scope -- consecutive rows in consecutive threads, so the column loads are coalesced and independent --
+  // and stores the loop's exports as packed bits in shared memory (ceil(exports / 32) words per row; bit k of word k / 32 = the
+  // loop's k-th export), together with the tile's slice of every used nested scope's CSR offsets (tile-relative).  The per-tile layout follows from the rows of every scope in the
   // tile (tile_lo): a header of region offsets, then the regions.  SpecSource::stage lists them so the launch can size the area.
   std::vector<uint32_t> nested;   // used nested scopes: their offsets are staged
   for (size_t s = 1; s < NS; ++s)
     if (g.scope_used[s]) nested.push_back((uint32_t)s);
   const uint32_t NG = (uint32_t)groups.size(), NR = NG + (uint32_t)nested.size(), data0 = (NR + 3u) & ~3u;
   auto group_scope = [&](size_t gi) { return g.atoms[groups[gi][0]].scope; };
-  auto group_words = [&](size_t gi) { return (uint32_t)((groups[gi].size() + 31) / 32); };
-  auto parent_of = [&](uint32_t s) { return (uint32_t)c.schema.scopes[s].parent; };
-  for (size_t gi = 0; gi < NG; ++gi) out.stage.push_back({group_scope(gi), group_words(gi), 0u});
+  auto group_words = [&](size_t gi) { return (uint32_t)((exports[gi].size() + 31) / 32); };
+  for (size_t gi = 0; gi < NG; ++gi) {
+    out.stage.push_back({group_scope(gi), group_words(gi), 0u});
+    out.fold.push_back({group_scope(gi), (uint32_t)groups[gi].size(), (uint32_t)gates[gi].size(), nany[gi], (uint32_t)exports[gi].size() - nany[gi]});
+  }
   for (uint32_t s : nested) out.stage.push_back({parent_of(s), 1u, 1u});
   out.stage_hdr = data0;
   std::ostringstream lay;   // the per-tile layout: b<s> / c<s> = first row / rows of scope s in the tile, R<g> / Q<s> = region offsets
@@ -794,7 +884,7 @@ struct uint4 { uint32_t x, y, z, w; };
     std::map<uint32_t, uint32_t> need;
     for (uint32_t ai : members)
       for (auto& kv : g.atoms[ai].need) need[kv.first] |= kv.second;
-    o << "    if (k < c" << s << ") {   // atoms of scope " << s << " (row loop " << gi << ")\n      const size_t row = (size_t)b" << s << " + k;\n";
+    o << "    if (k < c" << s << ") {   // atoms, row-local gates and exports of scope " << s << " (row loop " << gi << ")\n      const size_t row = (size_t)b" << s << " + k;\n";
     for (auto& kv : need) {
       const uint32_t ci = kv.first, enc = kv.second;
       const std::string K = std::to_string(ci);
@@ -805,10 +895,21 @@ struct uint4 { uint32_t x, y, z, w; };
         o << "      const uint4* __restrict__ ph" << K << " = reinterpret_cast<const uint4*>(cols[" << K << "].head);\n      const uint4 h" << K << "a = GK_SPEC_LD(ph" << K
           << " + 2 * row), h" << K << "b = GK_SPEC_LD(ph" << K << " + 2 * row + 1);\n";
     }
+    for (uint32_t ai : members) o << "      const bool v" << g.atoms[ai].var << " = " << g.atoms[ai].expr << ";\n";
+    for (uint32_t v : gates[gi]) {
+      const SpecNode& n = g.nodes[(size_t)g.producer[v]];
+      std::string e;
+      for (const auto& in : n.in) {
+        const bool k = in.first < 0 || konst[(size_t)in.first] >= 0;
+        const std::string x = k ? ((in.first >= 0 && konst[(size_t)in.first] == 1) ? "true" : "false") : "v" + std::to_string(in.first);
+        e += (e.empty() ? "" : n.is_or ? " | " : " & ") + std::string(in.second ? "!" : "") + x;
+      }
+      o << "      const bool v" << v << " = " << (n.neg_out ? "!(" + e + ")" : e) << ";   // row-local gate\n";
+    }
     o << "      uint32_t";
     for (uint32_t w = 0; w < AW; ++w) o << (w ? ", a" : " a") << w << " = 0u";
     o << ";\n";
-    for (size_t m = 0; m < members.size(); ++m) o << "      if (" << g.atoms[members[m]].expr << ") a" << m / 32 << " |= " << hx(1u << (m % 32)) << ";\n";
+    for (size_t m = 0; m < exports[gi].size(); ++m) o << "      if (v" << exports[gi][m] << ") a" << m / 32 << " |= " << hx(1u << (m % 32)) << ";\n";
     for (uint32_t w = 0; w < AW; ++w) o << "      stg[R" << gi << " + " << AW << "u * k + " << w << "u] = a" << w << ";\n";
     o << "      continue;\n    }\n    k -= c" << s << ";\n";
   }
@@ -836,29 +937,37 @@ struct uint4 { uint32_t x, y, z, w; };
     o << "  const uint32_t f" << s << " = n" << s << " >= 32u ? 0xffffffffu : ((1u << n" << s << ") - 1u);\n  (void)hi" << s << "; (void)f" << s << ";\n  big = big || r" << s
       << " > 32u;\n";
   }
-  std::vector<uint8_t> group_done(groups.size(), 0);
-  auto emit_group = [&](int gi) {
-    if (gi < 0 || group_done[(size_t)gi]) return;
-    group_done[(size_t)gi] = 1;
-    const std::vector<uint32_t>& members = groups[(size_t)gi];
-    const uint32_t s = group_scope((size_t)gi), AW = group_words((size_t)gi);
-    o << "  // ---- atoms of scope " << s << " (row loop " << gi << "): the bits gk_spec_stage() left for the object's rows\n";
+  std::vector<uint8_t> group_done(groups.size(), 0), any_done(g.nvar, 0);
+  auto emit_group = [&](size_t gi) {
+    if (group_done[gi]) return;
+    group_done[gi] = 1;
+    const std::vector<uint32_t>& ex = exports[gi];
+    const uint32_t s = group_scope(gi), AW = group_words(gi), AN = (nany[gi] + 31u) / 32u;
+    o << "  // ---- exports of scope " << s << " (row loop " << gi << "): the bits gk_spec_stage() left for the object's rows; x" << gi << "_<w> = the OR of the rows' words\n";
     o << "  const uint32_t* __restrict__ a" << gi << " = stg + stg[" << gi << "];\n";
-    o << "  uint32_t";
-    for (size_t k = 0; k < members.size(); ++k) o << (k ? ", v" : " v") << g.atoms[members[k]].var << " = 0u";
+    if (AN || ex.size() > nany[gi]) o << "  uint32_t";
+    for (uint32_t w = 0; w < AN; ++w) o << (w ? ", x" : " x") << gi << "_" << w << " = 0u";
+    for (size_t k = nany[gi]; k < ex.size(); ++k) o << (k || AN ? ", v" : " v") << ex[k] << " = 0u";
     o << ";\n";
     if (s == 0) o << "  {\n    const uint32_t row = o;\n    const uint32_t bit = 1u;\n";
     else o << "  _Pragma(\"unroll 1\") for (uint32_t j = 0; j < n" << s << "; ++j) {\n    const uint32_t row = lo" << s << " + j;\n    const uint32_t bit = 1u << j;\n";
-    o << "    const uint32_t";
+    o << "    (void)bit;\n    const uint32_t";
     for (uint32_t w = 0; w < AW; ++w) o << (w ? ", w" : " w") << w << " = a" << gi << "[" << AW << "u * row + " << w << "u]";
     o << ";\n";
-    for (size_t m = 0; m < members.size(); ++m) o << "    if (w" << m / 32 << " & " << hx(1u << (m % 32)) << ") v" << g.atoms[members[m]].var << " |= bit;\n";
+    for (uint32_t w = 0; w < AN; ++w) o << "    x" << gi << "_" << w << " |= w" << w << ";\n";
+    for (size_t k = nany[gi]; k < ex.size(); ++k) o << "    if (w" << k / 32 << " & " << hx(1u << (k % 32)) << ") v" << ex[k] << " |= bit;\n";
     o << "  }\n";
   };
-  // ---- everything else depth-first from the results: a node right after what it reads
+  // ---- everything else depth-first from the results: a node right after what it reads.  The gates phase 1 evaluated are not nodes
+  // here: the walk ends at the exports.
   std::function<void(uint32_t)> emit_var = [&](uint32_t v) {
-    if (g.atom_of[v] >= 0) {
-      emit_group(g.atoms[(size_t)g.atom_of[v]].group);
+    if (local[v] >= 0) {
+      const size_t gi = (size_t)group_ix.at((uint32_t)local[v]);
+      emit_group(gi);
+      if (form[v] == kAny && !any_done[v]) {   // (0 or 1: the object-level EXISTS that reads it tests `!= 0`)
+        any_done[v] = 1;
+        o << "  const uint32_t v" << v << " = (x" << gi << "_" << bit_of[v] / 32 << " >> " << bit_of[v] % 32 << ") & 1u;\n";
+      }
       return;
     }
     const int pr = g.producer[v];
@@ -886,7 +995,8 @@ struct uint4 { uint32_t x, y, z, w; };
   out.smem = r16(c.schema.cols.size() * sizeof(GkColumn) + NS * sizeof(GkScope) + 3 * (size_t)W * 32 * 4 + (size_t)W * 4) + 16;
   o << "#define GK_SPEC_NS " << NS << "u\n#define GK_SPEC_STAGE_AT " << out.smem << "u   /* the staging area's byte offset in dynamic shared memory */\n";
   o << kWrapper;
-  out.src = o.str();
+  // (the folding as the text's first line: a dumped text says what it stages)
+  out.src = "// " + out.fold_text() + "\n" + o.str();
   out.words = W;
   out.n_fast = g.n_fast;
   out.n_generic = g.n_generic;

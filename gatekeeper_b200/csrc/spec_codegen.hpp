@@ -2,10 +2,12 @@
 //
 // gk_eval_kernel (tile_kernel.cuh) INTERPRETS the netlist: every node is a bit column of a 512-object tile in shared memory, every
 // op a work item some warp decodes, ~400 warp-instructions per object at the benchmark's 50 constraints.  The netlist is known when
-// the constraint set is compiled, so the engine also writes it out as straight-line code -- one thread per object, every node a
-// 32-bit mask register (bit j = row j of THIS object in the node's scope), constants as immediates, EXISTS a `!= 0`, the
-// object-major bitmap words assembled in registers without a transpose -- and NVRTC compiles that text for sm_90a when the first
-// large batch is evaluated (kernels.cu).  Objects with more than 32 rows in some scope do not fit the mask registers: their tiles
+// the constraint set is compiled, so the engine also writes it out as straight-line code, constants as immediates, in two phases per
+// tile.  Phase 1, one thread per ROW: the row's atoms and every gate that reads that row alone, of which only the bits something
+// else reads (exports) are stored in shared memory.  Phase 2, one thread per OBJECT: every remaining node a 32-bit mask register
+// (bit j = row j of THIS object in the node's scope), an export that only object-level EXISTS read one bit of the OR of the rows'
+// words, EXISTS a `!= 0`, the object-major bitmap words assembled in registers without a transpose.  NVRTC compiles that text for
+// sm_90a when the first large batch is evaluated (kernels.cu).  Objects with more than 32 rows in some scope do not fit the mask registers: their tiles
 // are handed to the interpreter (GkKParams::tile_list).
 #pragma once
 #include <string>
@@ -26,6 +28,21 @@ struct SpecSource {
   };
   std::vector<StageRegion> stage;
   uint32_t stage_hdr = 0;
+  // per scope with atoms: what phase 1 evaluates on a row (atoms, row-local gates) and what it stages of it (exports, by read form)
+  struct Fold {
+    uint32_t scope, atoms, gates, any, mask;
+  };
+  std::vector<Fold> fold;
+  // "folded: scope S: A atoms + G gates -> X any + Y mask in W words; ..." (the first line of `src`, and the backend's trace)
+  std::string fold_text() const {
+    std::string t = "folded:";
+    for (size_t i = 0; i < fold.size(); ++i) {
+      const Fold& f = fold[i];
+      t += std::string(i ? ";" : "") + " scope " + std::to_string(f.scope) + ": " + std::to_string(f.atoms) + " atoms + " + std::to_string(f.gates) + " gates -> " +
+           std::to_string(f.any) + " any + " + std::to_string(f.mask) + " mask in " + std::to_string(stage[i].per_row) + " words";
+    }
+    return t;
+  }
   // bytes of the staging area for a batch whose largest tile has cap[s] rows in scope s
   size_t stage_bytes(const std::vector<uint32_t>& cap) const {
     size_t w = stage_hdr;

@@ -2,7 +2,7 @@
 print the static picture: registers, spills, SASS instruction count, instructions per source region.  No GPU needed (NVRTC and
 cuobjdump / nvdisasm run in the authoring container); these are static numbers, never a timing.
 
-    python tools/spec_nvrtc.py /tmp/spec/config2.cu [--threads 256] [--minb 2] [--defs "-DGK_SPEC_X_NOMATCH"]
+    python tools/spec_nvrtc.py /tmp/spec/config2.cu [--threads 256] [--minb 3] [--defs "-DGK_SPEC_X_NOMATCH"]
 """
 import argparse
 import collections
@@ -14,7 +14,7 @@ import sys
 import time
 
 
-def nvrtc_compile(src: bytes, threads=256, minb=2, defs=()):
+def nvrtc_compile(src: bytes, threads=256, minb=3, defs=()):
     """-> (cubin bytes, log text, seconds).  Raises RuntimeError with the log when the text does not compile."""
     h = None
     for name in ("libnvrtc.so.12", "/usr/local/cuda/lib64/libnvrtc.so.12", "libnvrtc.so", "/usr/local/cuda/lib64/libnvrtc.so"):
@@ -73,7 +73,13 @@ def static_report(cubin_path: str, cu_path: str):
             if cur is None:
                 region["?"] += 1
             elif stage <= cur < start:
-                region["stage: atom bits and offsets of the tile's rows (phase 1)"] += 1
+                s = src[cur - 1].strip()
+                if s.endswith("// row-local gate"):
+                    region["stage: row-local gates"] += 1
+                elif re.match(r"if \(v\d+\) a\d+ \|= ", s) or re.match(r"stg\[R\d+ ", s):
+                    region["stage: export bits packed and stored"] += 1
+                else:
+                    region["stage: loads, atoms, offsets, control"] += 1
             elif cur < start:
                 region["spec.match (written-out blocks / vm_core.h)"] += 1
             elif cur < end:
@@ -81,7 +87,9 @@ def static_report(cubin_path: str, cu_path: str):
                 if "rm =" in s or s.startswith("for (uint32_t pj") or "pj" in s:
                     region["object: EXISTS / broadcast range loops"] += 1
                 elif s.startswith("if (") and "|= bit" in s:
-                    region["object: atom tests"] += 1
+                    region["object: export bits, mask form"] += 1
+                elif re.match(r"x\d+_\d+ \|= w\d+;", s) or re.match(r"const uint32_t v\d+ = \(x\d+_\d+ >> ", s):
+                    region["object: export bits, any form"] += 1
                 elif "GK_SPEC_LD(p" in s or "_Pragma" in s or "bit = " in s or re.search(r"\bw0 = a\d+\[", s):
                     region["object: row loops (loads, control)"] += 1
                 elif "GK_SPEC_MATCH" in s or "GK_SPEC_ERR" in s:
@@ -99,7 +107,7 @@ if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("cu")
     ap.add_argument("--threads", type=int, default=256)
-    ap.add_argument("--minb", type=int, default=2)
+    ap.add_argument("--minb", type=int, default=3)
     ap.add_argument("--defs", default="")
     a = ap.parse_args()
     cubin, log, dt = nvrtc_compile(open(a.cu, "rb").read(), a.threads, a.minb, a.defs.split())
