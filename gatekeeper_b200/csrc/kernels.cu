@@ -70,6 +70,7 @@ struct DevBatch {
   bool gvk_uniform = false;   // every object that was not skipped has the same apiVersion and kind
   unsigned long long* gvk = nullptr;   // [n] hash of (apiVersion, kind) per object, 0 for a skipped one (audit_candidates)
   std::vector<uint32_t> cap;  // rows of the largest tile per scope (sizes the slot area of any netlist over this batch)
+  std::vector<uint32_t> rows; // rows per scope in the batch, rows[0] = objects (sizes the generated kernel's export arrays)
   bool fork = false;          // a view made by fork_batch: arena and tiling belong to the batch it was forked from
 };
 
@@ -278,6 +279,7 @@ class CudaBackend : public Backend {
     if (d_scalars_) cudaFree(d_scalars_);
     if (d_totals_) cudaFree(d_totals_);
     if (d_errlist_) cudaFree(d_errlist_);
+    if (d_spec_x_) cudaFree(d_spec_x_);
     if (d_active_) cudaFree(d_active_);
     if (pinned_) cudaFreeHost(pinned_);
     cudaEventDestroy(ev0_);
@@ -381,6 +383,9 @@ class CudaBackend : public Backend {
     db->tile = tile;
     db->prog_version = c.version;
     db->gvk_uniform = hb.gvk_hi == 0 || hb.gvk_lo == hb.gvk_hi;
+    db->rows = hb.scope_rows;
+    db->rows.resize(NS, 0);
+    db->rows[0] = hb.n;
     dmalloc(&db->arena, db->bytes);
     dmalloc(&db->d_tile_lo, tile_lo.size() * 4 + 64);
     if (hb.n) dmalloc(&db->gvk, (size_t)hb.n * 8);
@@ -596,6 +601,17 @@ class CudaBackend : public Backend {
         spec_per_sm_ = spec_minb_;
       }
       spec_per_sm_ = std::max(1, spec_per_sm_);
+      // the export arrays: scratch rewritten by every evaluation, grown (never shrunk) outside the timed region
+      const size_t xb = spec_cur_->src.export_bytes(db->rows);
+      if (spec_next_ && xb > spec_x_bytes_) {
+        if (d_spec_x_) CK(cudaFree(d_spec_x_));
+        d_spec_x_ = nullptr;
+        spec_x_bytes_ = 0;
+        CK(cudaMalloc(&d_spec_x_, xb));
+        spec_x_bytes_ = xb;
+        if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[spec] export arrays: %zu bytes for %u objects\n", xb, db->n);
+      }
+      spec_rows_grid_ = spec_cur_->src.rows_blocks(db->rows, (uint32_t)spec_cur_->rows_threads);
     }
 #ifdef GK_PHASE_TIMING
     if (!d_timing_) CK(cudaMalloc(&d_timing_, (kMaxPhases + 2 + 16) * 16));
@@ -636,9 +652,16 @@ class CudaBackend : public Backend {
       // the kernel generated for this constraint set does the tiles whose objects fit its mask registers (all of them, normally);
       // the interpreter behind it takes the tiles it listed and, in the fused exchange, publishes the totals of both
       SpecEntry& se = *spec_cur_;
-      void* args[] = {&p};
+      uint32_t* xs = d_spec_x_;
+      void* args[] = {&p, &xs};
+      // the rows kernel evaluates every row of the batch into the export arrays, one thread per row
+      if (spec_rows_grid_) {
+        CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.rows_kern), dim3(spec_rows_grid_), dim3((unsigned)se.rows_threads), args, 0, st));
+        ++launches_;
+      }
       // persistent CTAs, as many as are resident at once, walk the tiles with a grid stride: the per-CTA set-up (tables, enforcement
-      // mask) is paid once per CTA, and where two or more are resident one CTA's staging overlaps another's object walk
+      // mask) is paid once per CTA, and where two or more are resident one CTA's copy overlaps another's object walk.  (Launched as the
+      // rows kernel's programmatic dependent, so that this set-up overlaps the rows kernel's last blocks, it measured no faster.)
       const uint32_t spec_grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * spec_per_sm_)));
       CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.kern), dim3(spec_grid), dim3((unsigned)se.threads), args, spec_smem_, st));
       ++launches_;
@@ -656,8 +679,9 @@ class CudaBackend : public Backend {
     SpecSource src;
     int state = 0;            // 0 = not compiled yet, 1 = ready, -1 = failed (the interpreter runs; reported once on stderr)
     cudaLibrary_t lib = nullptr;
-    cudaKernel_t kern = nullptr;
-    int threads = 128;
+    cudaKernel_t kern = nullptr;        // gk_spec_kernel
+    cudaKernel_t rows_kern = nullptr;   // gk_spec_rows_kernel
+    int threads = 128, rows_threads = 256;
     size_t max_smem = 0;      // dynamic shared memory the kernel may be launched with (fixed part + the tile's staging area)
     double compile_ms = 0;
   };
@@ -713,14 +737,15 @@ class CudaBackend : public Backend {
       if (!create || !compile || !log_size || !get_log || !bin_size || !get_bin || !destroy) throw BackendError{"NVRTC entry points missing"};
       Prog prog = nullptr;
       if (create(&prog, se.src.src.c_str(), "gk_spec_kernel.cu", 0, nullptr, nullptr) != 0) throw BackendError{"nvrtcCreateProgram failed"};
-      const std::string threads = "-DGK_SPEC_THREADS=" + std::to_string(spec_threads_), minb = "-DGK_SPEC_MINB=" + std::to_string(spec_minb_);
+      const std::string threads = "-DGK_SPEC_THREADS=" + std::to_string(spec_threads_), minb = "-DGK_SPEC_MINB=" + std::to_string(spec_minb_),
+                        rthreads = "-DGK_SPEC_ROWS_THREADS=" + std::to_string(spec_rows_threads_), rminb = "-DGK_SPEC_ROWS_MINB=" + std::to_string(spec_rows_minb_);
       std::vector<std::string> extra;   // GK_SPEC_DEFS="-DX -DY": measurement switches of the generated text
       if (const char* d = getenv("GK_SPEC_DEFS")) {
         std::istringstream in(d);
         std::string tok;
         while (in >> tok) extra.push_back(tok);
       }
-      std::vector<const char*> opts = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device", threads.c_str(), minb.c_str()};
+      std::vector<const char*> opts = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device", threads.c_str(), minb.c_str(), rthreads.c_str(), rminb.c_str()};
       for (auto& x : extra) opts.push_back(x.c_str());
       const int rc = compile(prog, (int)opts.size(), opts.data());
       if (rc != 0) {
@@ -738,7 +763,9 @@ class CudaBackend : public Backend {
       destroy(&prog);
       CK(cudaLibraryLoadData(&se.lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0));
       CK(cudaLibraryGetKernel(&se.kern, se.lib, "gk_spec_kernel"));
+      CK(cudaLibraryGetKernel(&se.rows_kern, se.lib, "gk_spec_rows_kernel"));
       se.threads = spec_threads_;
+      se.rows_threads = spec_rows_threads_;
       cudaFuncAttributes fa;
       CK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(se.kern)));
       se.max_smem = optin_smem_ - fa.sharedSizeBytes;
@@ -1177,6 +1204,8 @@ class CudaBackend : public Backend {
     std::unique_ptr<DevBatch, std::function<void(DevBatch*)>> guard(db, [this](DevBatch* x) { release(x); });
     db->bytes = gk_align(ac.off);
     db->n = n;
+    db->rows = total;
+    db->rows[0] = n;
     db->prog_version = c.version;
     dmalloc(&db->arena, db->bytes);
     uint8_t* A = db->arena;
@@ -1431,6 +1460,7 @@ class CudaBackend : public Backend {
     f->tile = db->tile;
     f->gvk_uniform = db->gvk_uniform;
     f->gvk = db->gvk;
+    f->rows = db->rows;
     f->fork = true;
     f->prog_version = other.version;
     std::unique_ptr<DevBatch, std::function<void(DevBatch*)>> guard(f, [this](DevBatch* x) { release(x); });
@@ -1750,6 +1780,12 @@ class CudaBackend : public Backend {
   int spec_threads_ = getenv("GK_SPEC_THREADS") ? std::min(1024, std::max(32, atoi(getenv("GK_SPEC_THREADS")) / 32 * 32)) : 256;
   int spec_minb_ = getenv("GK_SPEC_MINB") ? std::max(1, atoi(getenv("GK_SPEC_MINB"))) : 3;   // 256 x 3: an 80-register cap, measured best or level at configs 2, 4 and 5 (DESIGN 5a)
   const char* last_kernel_ = "gk_eval_kernel";
+  // gk_spec_rows_kernel: one thread per row, no shared memory
+  int spec_rows_threads_ = getenv("GK_SPEC_ROWS_THREADS") ? std::min(1024, std::max(32, atoi(getenv("GK_SPEC_ROWS_THREADS")) / 32 * 32)) : 256;
+  int spec_rows_minb_ = getenv("GK_SPEC_ROWS_MINB") ? std::max(1, atoi(getenv("GK_SPEC_ROWS_MINB"))) : 6;   // 256 x 6: a 40-register cap, no spill at config 2 (DESIGN 5a)
+  uint32_t* d_spec_x_ = nullptr;   // the export arrays (SpecSource::export_bytes), grow-only
+  size_t spec_x_bytes_ = 0;
+  uint32_t spec_rows_grid_ = 0;    // blocks of the next rows-kernel launch (set with spec_next_)
   bool spec_next_ = false;
   size_t spec_smem_ = 0;      // dynamic shared memory of the next launch of the generated kernel (set with spec_next_)
   int spec_per_sm_ = 1;       // its resident CTAs per SM at that size

@@ -52,7 +52,7 @@ __device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
   return x;
 }
 
-extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_spec_kernel(const __grid_constant__ GkKParams p) {
+extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_spec_kernel(const __grid_constant__ GkKParams p, const uint32_t* __restrict__ xs) {
   extern __shared__ uint4 gk_smem4[];
   unsigned char* smem = reinterpret_cast<unsigned char*>(gk_smem4);
   const uint32_t NC = p.batch.ncols, NS = p.batch.nscopes;
@@ -88,10 +88,10 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
   for (uint32_t w = 0; w < GK_SPEC_W; ++w) tv[w] = te[w] = 0u;
   for (uint32_t t = blockIdx.x; t < p.ntiles; t += gridDim.x) {
     const uint32_t obj0 = t * p.tile, nobj = min(p.tile, p.batch.n - obj0);
-    // phase 1: the tile's rows, every thread of the CTA; phase 2: its objects, one per thread.  (The barrier at the end of the tile
-    // keeps the next tile's staging from overwriting what the last objects of this one still read.)
+    // phase 1: the copy of the tile's exports and offsets, every thread of the CTA; phase 2: its objects, one per thread.  (The
+    // barrier at the end of the tile keeps the next tile's copy from overwriting what the last objects of this one still read.)
     const uint32_t* tl = p.tile_lo + (size_t)t * NS;
-    gk_spec_stage(p.batch, cols, scopes, p.prog.pool, p.prog.cbytes, tl, tl + NS, stg, threadIdx.x, blockDim.x);
+    gk_spec_stage(p.batch, scopes, xs, tl, tl + NS, stg, threadIdx.x, blockDim.x);
     __syncthreads();
     // An object with more rows in a scope than a mask register holds makes gk_spec_object() return true: the tile is then listed
     // for the interpreter, which evaluates it again and overwrites what this kernel stored for it; its totals are not counted here.
@@ -99,7 +99,11 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
     uint32_t tvt[GK_SPEC_W], tet[GK_SPEC_W];
 #pragma unroll
     for (uint32_t w = 0; w < GK_SPEC_W; ++w) tvt[w] = tet[w] = 0u;
+#ifdef GK_SPEC_X_STAGEONLY   /* (measurement only: the staging of every tile without the object walk; results differ) */
+    for (uint32_t base = nobj; base < nobj; base += blockDim.x) {
+#else
     for (uint32_t base = 0; base < nobj; base += blockDim.x) {
+#endif
       const uint32_t o = base + threadIdx.x;
       uint32_t vw[GK_SPEC_W], ew[GK_SPEC_W];
 #pragma unroll
@@ -163,8 +167,9 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
 #else
 #include <vector>
 // TEST-ONLY host build (tests/_hostemu, GK_SPEC_CHECK=1): one object; returns 1 when the object does not fit the mask registers.
-// The object's tile (GK_SPEC_HOST_TILE objects; its rows found through the CSR offsets) is staged by the same gk_spec_stage() the
-// kernel runs, with three "threads" striding over its rows, and staged again only when `obj` leaves it (or starts it again).
+// The rows of the object's tile (GK_SPEC_HOST_TILE objects; its rows found through the CSR offsets) are evaluated by the same
+// gk_spec_row_<g>() the rows kernel runs into a poisoned export buffer, which the same gk_spec_stage() the tile kernel runs copies
+// with three "threads" striding over it; both again only when `obj` leaves the tile (or starts it again).
 #ifndef GK_SPEC_HOST_TILE
 #define GK_SPEC_HOST_TILE 96u
 #endif
@@ -176,7 +181,7 @@ extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint
   struct Tile {
     const void* flags = nullptr;
     uint32_t n = 0, t = 0xffffffffu;
-    std::vector<uint32_t> lo, hi, stg;
+    std::vector<uint32_t> lo, hi, stg, x;
   };
   static thread_local Tile k;
   const GkBatch& B = p->batch;
@@ -188,7 +193,9 @@ extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint
     k.hi[0] = B.n - t * T < T ? B.n : (t + 1u) * T;
     gk_spec_tile_rows(B.scopes, k.lo.data(), k.hi.data());
     k.stg.assign(gk_spec_stage_words(k.lo.data(), k.hi.data()), 0xdeadbeefu);   // (poisoned: a word the staging misses shows)
-    for (uint32_t tid = 0; tid < 3u; ++tid) gk_spec_stage(B, B.cols, B.scopes, p->prog.pool, p->prog.cbytes, k.lo.data(), k.hi.data(), k.stg.data(), tid, 3u);
+    k.x.assign(gk_spec_export_words(B), 0xdeadbeefu);
+    gk_spec_host_rows(p, k.lo.data(), k.hi.data(), k.x.data());
+    for (uint32_t tid = 0; tid < 3u; ++tid) gk_spec_stage(B, B.scopes, k.x.data(), k.lo.data(), k.hi.data(), k.stg.data(), tid, 3u);
     k.flags = B.flags;
     k.n = B.n;
     k.t = t;
@@ -412,6 +419,10 @@ struct Gen {
   uint32_t nvar = 0;
   size_t n_fast = 0, n_generic = 0;
   std::set<uint32_t> match_used;
+  struct MatchRec {
+    uint32_t vm, ve, mid;                  // match bit, error bit, block
+  };
+  std::vector<MatchRec> matches;
   std::ostringstream body;                 // the node being built
   std::vector<uint32_t> deps;
 
@@ -620,10 +631,9 @@ struct Gen {
       case GK_N_MATCH: {
         const uint32_t mid = op.w2;
         match_used.insert(mid);
+        // (no text here: the block is evaluated on the object's scope-0 row, and its two bits are exports of that row)
         const uint32_t vm = fresh(out), ve = fresh(op.w1 & 0xffffu);
-        body << "  const int m" << vm << " = skip ? 0 : GK_SPEC_MATCH(" << mid << ", B, pool, cbytes, obj);\n";
-        body << "  if (m" << vm << " < 0) GK_SPEC_ERR(obj, " << mid << "u, (uint32_t)(-m" << vm << "));\n";
-        body << "  const uint32_t v" << vm << " = m" << vm << " > 0 ? 1u : 0u, v" << ve << " = m" << vm << " < 0 ? 1u : 0u;\n";
+        matches.push_back({vm, ve, mid});
         break;
       }
       default: break;
@@ -649,6 +659,7 @@ SpecSource spec_codegen(const Compiled& c) {
   o << "// generated by spec_codegen.cpp for constraint-set version " << c.version << ": " << C << " constraints, " << c.ops.size() << " netlist ops\n";
   o << "#define GK_SPEC_C " << C << "u\n#define GK_SPEC_W " << W << "\n";
   o << "#ifndef GK_SPEC_THREADS\n#define GK_SPEC_THREADS 256\n#endif\n#ifndef GK_SPEC_MINB\n#define GK_SPEC_MINB 3\n#endif\n";
+  o << "#ifndef GK_SPEC_ROWS_THREADS\n#define GK_SPEC_ROWS_THREADS 256\n#endif\n#ifndef GK_SPEC_ROWS_MINB\n#define GK_SPEC_ROWS_MINB 6\n#endif\n";
   o << "#ifndef GK_SPEC_HOST\n#define GK_LD(p) __ldg(p)   /* pool, cbytes and every batch array are global and read-only here */\n#endif\n";
   o << strip_includes(kSpecHdrProgram) << strip_includes(kSpecHdrVmCore);
   o << R"GKSRC(
@@ -671,10 +682,15 @@ SpecSource spec_codegen(const Compiled& c) {
     }                                                                \
   }
 struct uint4 { uint32_t x, y, z, w; };
+#define GK_SPEC_CP4(d, s) (*(d) = *(s))
+#define GK_SPEC_CP_WAIT()
 #else
 #define GK_SPEC_FN __device__ __forceinline__
 #define GK_SPEC_LD(p) __ldg(p)      /* every array of a resident batch is read-only while it is evaluated */
 #define GK_SPEC_POPC(x) __popc(x)
+/* one 4-byte global -> shared copy in flight (the export slices are 4-byte aligned only); GK_SPEC_CP_WAIT() lands this thread's */
+#define GK_SPEC_CP4(d, s) asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((uint32_t)__cvta_generic_to_shared(d)), "l"(s) : "memory")
+#define GK_SPEC_CP_WAIT() asm volatile("cp.async.wait_all;\n" ::: "memory")
 #define GK_SPEC_ERR(o, mid, code)                                    \
   {                                                                  \
     const uint32_t sl_ = atomicAdd(out.errcount, 1u);                \
@@ -743,21 +759,26 @@ struct uint4 { uint32_t x, y, z, w; };
   // better: every extra loop is one more exposed memory latency per object.
   std::map<uint32_t, int> group_ix;   // scope -> row loop
   std::vector<std::vector<uint32_t>> groups;
+  std::vector<uint32_t> gscope;       // row loop -> its scope
+  auto add_group = [&](uint32_t s) {
+    auto it = group_ix.find(s);
+    if (it != group_ix.end()) return it->second;
+    group_ix.emplace(s, (int)groups.size());
+    groups.emplace_back();
+    gscope.push_back(s);
+    return (int)groups.size() - 1;
+  };
   for (const Ord& e : order) {
     const GkOutEnt& oe = c.outs[e.cix];
     if ((oe.flags & 3u) || var_of(oe.prog_slot) < 0) continue;
     for (uint32_t ai : cone((uint32_t)var_of(oe.prog_slot))) {
       Gen::AtomRec& r = g.atoms[ai];
       if (r.group >= 0) continue;
-      auto it = group_ix.find(r.scope);
-      if (it == group_ix.end()) {
-        it = group_ix.emplace(r.scope, (int)groups.size()).first;
-        groups.emplace_back();
-      }
-      r.group = it->second;
+      r.group = add_group(r.scope);
       groups[(size_t)r.group].push_back(ai);
     }
   }
+  if (!g.matches.empty()) add_group(0);   // the match blocks are evaluated on the scope-0 row, with or without atoms there
   auto parent_of = [&](uint32_t s) { return (uint32_t)c.schema.scopes[s].parent; };
   // ---- row-local values and exports.  A variable of scope L is ROW-LOCAL when it is a function of one row of L alone: an atom of L,
   // or a gate of L whose inputs are row-local values and constants (and at least one of the former).  Phase 1 has every atom of a
@@ -769,9 +790,15 @@ struct uint4 { uint32_t x, y, z, w; };
   enum : uint8_t { kNotExported = 0, kAny = 1, kMask = 2 };
   std::vector<int> local(g.nvar, -1);      // variable -> the scope it is row-local in
   std::vector<int8_t> konst(g.nvar, -1);   // variable -> its value in a row that exists, when it is a constant
+  std::vector<uint8_t> is_match(g.nvar, 0);   // the match / error bit of a spec.match block: row-local in scope 0
+  for (const Gen::MatchRec& m : g.matches) is_match[m.vm] = is_match[m.ve] = 1;
   for (uint32_t v = 0; v < g.nvar; ++v) {
     if (g.atom_of[v] >= 0) {
       local[v] = (int)g.atoms[(size_t)g.atom_of[v]].scope;
+      continue;
+    }
+    if (is_match[v]) {
+      local[v] = 0;
       continue;
     }
     if (g.producer[v] < 0) continue;
@@ -791,7 +818,7 @@ struct uint4 { uint32_t x, y, z, w; };
     if (all && some) local[v] = (int)n.level;
     else if (all) konst[v] = (val != n.neg_out) ? 1 : 0;
   }
-  auto folded = [&](uint32_t v) { return local[v] >= 0 && g.atom_of[v] < 0; };   // a gate phase 1 evaluates
+  auto folded = [&](uint32_t v) { return local[v] >= 0 && g.atom_of[v] < 0 && !is_match[v]; };   // a gate phase 1 evaluates
   std::vector<uint8_t> form(g.nvar, kNotExported), live(g.nvar, 0);
   {
     std::vector<uint32_t> todo;
@@ -834,23 +861,28 @@ struct uint4 { uint32_t x, y, z, w; };
     }
   for (uint32_t v = 0; v < g.nvar; ++v)
     if (live[v] && folded(v)) gates[(size_t)group_ix.at((uint32_t)local[v])].push_back(v);
-  // ---- phase 1, gk_spec_stage(): once per tile the whole CTA evaluates the atoms and the row-local gates of every row loop on every
-  // row of the tile in that scope -- consecutive rows in consecutive threads, so the column loads are coalesced and independent --
-  // and stores the loop's exports as packed bits in shared memory (ceil(exports / 32) words per row; bit k of word k / 32 = the
-  // loop's k-th export), together with the tile's slice of every used nested scope's CSR offsets (tile-relative).  The per-tile layout follows from the rows of every scope in the
-  // tile (tile_lo): a header of region offsets, then the regions.  SpecSource::stage lists them so the launch can size the area.
+  // ---- the rows, gk_spec_row_<g>() run by gk_spec_rows_kernel: one thread per row of a row loop's scope over the whole batch evaluates
+  // the loop's atoms and row-local gates (on a scope-0 row also the spec.match blocks, listing their errors) and stores the loop's
+  // exports as packed bits to the loop's EXPORT ARRAY in global memory, indexed by the row's batch index (ceil(exports / 32) words
+  // per row; bit k of word k / 32 = the loop's k-th export).  The arrays lie back to back in one scratch buffer, in row-loop order,
+  // each sized by its scope's rows in the batch (SpecSource::export_bytes).
+  // ---- the tile, gk_spec_stage(): the CTA copies the tile's slice of every export array, and of every used nested scope's CSR offsets
+  // (tile-relative), into shared memory.  The per-tile layout follows from the rows of every scope in the tile (tile_lo): a header
+  // of region offsets, then the regions.  SpecSource::stage lists them so the launch can size the area.
   std::vector<uint32_t> nested;   // used nested scopes: their offsets are staged
   for (size_t s = 1; s < NS; ++s)
     if (g.scope_used[s]) nested.push_back((uint32_t)s);
   const uint32_t NG = (uint32_t)groups.size(), NR = NG + (uint32_t)nested.size(), data0 = (NR + 3u) & ~3u;
-  auto group_scope = [&](size_t gi) { return g.atoms[groups[gi][0]].scope; };
+  auto group_scope = [&](size_t gi) { return gscope[gi]; };
   auto group_words = [&](size_t gi) { return (uint32_t)((exports[gi].size() + 31) / 32); };
   for (size_t gi = 0; gi < NG; ++gi) {
     out.stage.push_back({group_scope(gi), group_words(gi), 0u});
-    out.fold.push_back({group_scope(gi), (uint32_t)groups[gi].size(), (uint32_t)gates[gi].size(), nany[gi], (uint32_t)exports[gi].size() - nany[gi]});
+    if (!groups[gi].empty())
+      out.fold.push_back({group_scope(gi), (uint32_t)groups[gi].size(), (uint32_t)gates[gi].size(), nany[gi], (uint32_t)exports[gi].size() - nany[gi], group_words(gi)});
   }
   for (uint32_t s : nested) out.stage.push_back({parent_of(s), 1u, 1u});
   out.stage_hdr = data0;
+  out.ngroups = NG;
   std::ostringstream lay;   // the per-tile layout: b<s> / c<s> = first row / rows of scope s in the tile, R<g> / Q<s> = region offsets
   lay << "  const uint32_t b0 = GK_SPEC_LD(tlo), c0 = GK_SPEC_LD(thi) - b0;\n  (void)b0; (void)c0;\n";
   for (uint32_t s : nested)
@@ -858,44 +890,50 @@ struct uint4 { uint32_t x, y, z, w; };
   lay << "  uint32_t at = " << data0 << "u;\n";
   for (size_t gi = 0; gi < NG; ++gi) lay << "  const uint32_t R" << gi << " = at;\n  at += c" << group_scope(gi) << " * " << group_words(gi) << "u;\n";
   for (uint32_t s : nested) lay << "  const uint32_t Q" << s << " = at;\n  at += c" << parent_of(s) << " + 1u;\n";
-  o << "\n#ifdef GK_SPEC_HOST\n";
-  o << "static uint32_t gk_spec_stage_words(const uint32_t* tlo, const uint32_t* thi) {\n" << lay.str() << "  return at;\n}\n";
-  o << "static void gk_spec_tile_rows(const GkScope* scopes, uint32_t* tlo, uint32_t* thi) {\n";
-  for (uint32_t s : nested)
-    o << "  tlo[" << s << "] = scopes[" << s << "].off[tlo[" << parent_of(s) << "]];\n  thi[" << s << "] = scopes[" << s << "].off[thi[" << parent_of(s) << "]];\n";
-  o << "}\n#endif\n";
-  o << "GK_SPEC_FN void gk_spec_stage(const GkBatch& B, const GkColumn* cols, const GkScope* scopes, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes,\n"
-       "                              const uint32_t* tlo, const uint32_t* thi, uint32_t* stg, const uint32_t tid, const uint32_t nthr) {\n"
-       "  (void)B; (void)cols; (void)scopes; (void)pool; (void)cbytes;\n";
-  o << lay.str();
-  o << "  if (tid == 0u) {\n";
-  for (size_t gi = 0; gi < NG; ++gi) o << "    stg[" << gi << "] = R" << gi << ";\n";
-  for (size_t j = 0; j < nested.size(); ++j) o << "    stg[" << NG + j << "] = Q" << nested[j] << ";\n";
-  // the offsets of sibling scopes are read at the same parent rows: one item stages all of a parent's children (independent loads)
-  std::map<uint32_t, std::vector<uint32_t>> children;
-  for (uint32_t s : nested) children[parent_of(s)].push_back(s);
-  o << "  }\n  const uint32_t total = 0u";
-  for (size_t gi = 0; gi < NG; ++gi) o << " + c" << group_scope(gi);
-  for (auto& ch : children) o << " + c" << ch.first << " + 1u";
-  o << ";\n  _Pragma(\"unroll 1\") for (uint32_t i = tid; i < total; i += nthr) {\n    uint32_t k = i;\n";
+  // X<g> = the word offset of row loop g's export array in the scratch buffer; X<NG> = the buffer's words
+  std::ostringstream xbase;
+  xbase << "  const size_t X0 = 0u;\n";
+  for (size_t gi = 0; gi < NG; ++gi) {
+    const uint32_t s = group_scope(gi);
+    xbase << "  const size_t X" << gi + 1 << " = X" << gi << " + " << (s ? "(size_t)scopes[" + std::to_string(s) + "].rows" : std::string("(size_t)B.n")) << " * "
+          << group_words(gi) << "u;\n";
+  }
+  xbase << "  (void)scopes;";
+  for (size_t gi = 0; gi <= NG; ++gi) xbase << " (void)X" << gi << ";";
+  xbase << "\n";
+  std::map<uint32_t, std::vector<const Gen::MatchRec*>> match_at;   // (only the blocks whose bits something reads)
+  for (const Gen::MatchRec& m : g.matches)
+    if (live[m.vm] || live[m.ve]) match_at[0].push_back(&m);
   for (size_t gi = 0; gi < NG; ++gi) {
     const std::vector<uint32_t>& members = groups[gi];
     const uint32_t s = group_scope(gi), AW = group_words(gi);
     std::map<uint32_t, uint32_t> need;
     for (uint32_t ai : members)
       for (auto& kv : g.atoms[ai].need) need[kv.first] |= kv.second;
-    o << "    if (k < c" << s << ") {   // atoms, row-local gates and exports of scope " << s << " (row loop " << gi << ")\n      const size_t row = (size_t)b" << s << " + k;\n";
+    o << "\n// atoms, row-local gates" << (s == 0 && !match_at[0].empty() ? ", spec.match blocks" : "") << " and exports of one row of scope " << s << " (row loop " << gi << ")\n";
+    o << "GK_SPEC_FN void gk_spec_row_" << gi << "(const GkBatch& B, const GkColumn* cols, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes, const GkOut& out,\n"
+      << "                              const size_t row, uint32_t* __restrict__ xg) {\n  (void)B; (void)cols; (void)pool; (void)cbytes; (void)out;\n";
     for (auto& kv : need) {
       const uint32_t ci = kv.first, enc = kv.second;
       const std::string K = std::to_string(ci);
-      if (enc & GK_ENC_VT) o << "      const uint32_t t" << K << " = GK_SPEC_LD(cols[" << K << "].vt + row);\n";
-      if (enc & GK_ENC_SID) o << "      const uint32_t i" << K << " = GK_SPEC_LD(cols[" << K << "].sid + row);\n";
-      if (enc & GK_ENC_NUM) o << "      const long long n" << K << " = GK_SPEC_LD(reinterpret_cast<const long long*>(cols[" << K << "].num) + row);\n";
+      if (enc & GK_ENC_VT) o << "  const uint32_t t" << K << " = GK_SPEC_LD(cols[" << K << "].vt + row);\n";
+      if (enc & GK_ENC_SID) o << "  const uint32_t i" << K << " = GK_SPEC_LD(cols[" << K << "].sid + row);\n";
+      if (enc & GK_ENC_NUM) o << "  const long long n" << K << " = GK_SPEC_LD(reinterpret_cast<const long long*>(cols[" << K << "].num) + row);\n";
       if (enc & GK_ENC_HEAD)
-        o << "      const uint4* __restrict__ ph" << K << " = reinterpret_cast<const uint4*>(cols[" << K << "].head);\n      const uint4 h" << K << "a = GK_SPEC_LD(ph" << K
+        o << "  const uint4* __restrict__ ph" << K << " = reinterpret_cast<const uint4*>(cols[" << K << "].head);\n  const uint4 h" << K << "a = GK_SPEC_LD(ph" << K
           << " + 2 * row), h" << K << "b = GK_SPEC_LD(ph" << K << " + 2 * row + 1);\n";
     }
-    for (uint32_t ai : members) o << "      const bool v" << g.atoms[ai].var << " = " << g.atoms[ai].expr << ";\n";
+    if (s == 0 && !match_at[0].empty()) {
+      // a skipped object (review-level error) evaluates no block and lists no error: both of its bits are 0
+      o << "  const uint32_t obj = (uint32_t)row;\n  const bool skip = (GK_SPEC_LD(B.flags + obj) & GK_F_SKIP) != 0u;\n";
+      for (const Gen::MatchRec* m : match_at[0]) {
+        const std::string M = std::to_string(m->vm);
+        o << "  const int m" << M << " = skip ? 0 : GK_SPEC_MATCH(" << m->mid << ", B, pool, cbytes, obj);\n";
+        o << "  if (m" << M << " < 0) GK_SPEC_ERR(obj, " << m->mid << "u, (uint32_t)(-m" << M << "));\n";
+        o << "  const bool v" << M << " = m" << M << " > 0, v" << m->ve << " = m" << M << " < 0;\n  (void)v" << M << "; (void)v" << m->ve << ";\n";
+      }
+    }
+    for (uint32_t ai : members) o << "  const bool v" << g.atoms[ai].var << " = " << g.atoms[ai].expr << ";\n";
     for (uint32_t v : gates[gi]) {
       const SpecNode& n = g.nodes[(size_t)g.producer[v]];
       std::string e;
@@ -904,30 +942,71 @@ struct uint4 { uint32_t x, y, z, w; };
         const std::string x = k ? ((in.first >= 0 && konst[(size_t)in.first] == 1) ? "true" : "false") : "v" + std::to_string(in.first);
         e += (e.empty() ? "" : n.is_or ? " | " : " & ") + std::string(in.second ? "!" : "") + x;
       }
-      o << "      const bool v" << v << " = " << (n.neg_out ? "!(" + e + ")" : e) << ";   // row-local gate\n";
+      o << "  const bool v" << v << " = " << (n.neg_out ? "!(" + e + ")" : e) << ";   // row-local gate\n";
     }
-    o << "      uint32_t";
+    o << "  uint32_t";
     for (uint32_t w = 0; w < AW; ++w) o << (w ? ", a" : " a") << w << " = 0u";
     o << ";\n";
-    for (size_t m = 0; m < exports[gi].size(); ++m) o << "      if (v" << exports[gi][m] << ") a" << m / 32 << " |= " << hx(1u << (m % 32)) << ";\n";
-    for (uint32_t w = 0; w < AW; ++w) o << "      stg[R" << gi << " + " << AW << "u * k + " << w << "u] = a" << w << ";\n";
-    o << "      continue;\n    }\n    k -= c" << s << ";\n";
+    for (size_t m = 0; m < exports[gi].size(); ++m) o << "  if (v" << exports[gi][m] << ") a" << m / 32 << " |= " << hx(1u << (m % 32)) << ";\n";
+    for (uint32_t w = 0; w < AW; ++w) o << "  xg[" << AW << "u * row + " << w << "u] = a" << w << ";\n";
+    o << "}\n";
   }
+  o << "\n#ifdef GK_SPEC_HOST\n";
+  o << "static uint32_t gk_spec_stage_words(const uint32_t* tlo, const uint32_t* thi) {\n" << lay.str() << "  return at;\n}\n";
+  o << "static void gk_spec_tile_rows(const GkScope* scopes, uint32_t* tlo, uint32_t* thi) {\n";
+  for (uint32_t s : nested)
+    o << "  tlo[" << s << "] = scopes[" << s << "].off[tlo[" << parent_of(s) << "]];\n  thi[" << s << "] = scopes[" << s << "].off[thi[" << parent_of(s) << "]];\n";
+  o << "}\n";
+  o << "static size_t gk_spec_export_words(const GkBatch& B) {\n  const GkScope* scopes = B.scopes;\n" << xbase.str() << "  return X" << NG << ";\n}\n";
+  // (the rows of the tile [tlo, thi) only: a copy that reads outside them finds the caller's poison)
+  o << "static void gk_spec_host_rows(const GkKParams* p, const uint32_t* tlo, const uint32_t* thi, uint32_t* xs) {\n  const GkBatch& B = p->batch;\n  const GkScope* scopes = B.scopes;\n"
+    << xbase.str();
+  for (size_t gi = 0; gi < NG; ++gi)
+    o << "  for (size_t row = tlo[" << group_scope(gi) << "]; row < thi[" << group_scope(gi) << "]; ++row) gk_spec_row_" << gi << "(B, B.cols, p->prog.pool, p->prog.cbytes, p->out, row, xs + X"
+      << gi << ");\n";
+  o << "}\n#else\n";
+  // one thread per row; blocks [first, first + ceil(rows / threads)) of the grid are row loop g's, so a block never mixes scopes
+  o << "extern \"C\" __global__ void __launch_bounds__(GK_SPEC_ROWS_THREADS, GK_SPEC_ROWS_MINB) gk_spec_rows_kernel(const __grid_constant__ GkKParams p, uint32_t* __restrict__ xs) {\n"
+    << "  const GkBatch& B = p.batch;\n  const GkScope* scopes = B.scopes;\n"
+    << xbase.str() << "  uint32_t blk = blockIdx.x;\n";
+  for (size_t gi = 0; gi < NG; ++gi) {
+    const uint32_t s = group_scope(gi);
+    o << "  {\n    const uint32_t nr = " << (s ? "scopes[" + std::to_string(s) + "].rows" : std::string("B.n")) << ", nb = (nr + GK_SPEC_ROWS_THREADS - 1u) / GK_SPEC_ROWS_THREADS;\n"
+      << "    if (blk < nb) {\n      const uint32_t row = blk * GK_SPEC_ROWS_THREADS + threadIdx.x;\n      if (row < nr) gk_spec_row_" << gi
+      << "(B, B.cols, p.prog.pool, p.prog.cbytes, p.out, row, xs + X" << gi << ");\n      return;\n    }\n    blk -= nb;\n  }\n";
+  }
+  o << "}\n#endif\n";
+  // the copy: every 4-byte copy of the export slices in flight (cp.async) before the offsets' loads
+  o << "GK_SPEC_FN void gk_spec_stage(const GkBatch& B, const GkScope* scopes, const uint32_t* __restrict__ xs, const uint32_t* tlo, const uint32_t* thi, uint32_t* stg,\n"
+       "                              const uint32_t tid, const uint32_t nthr) {\n  (void)B; (void)xs;\n";
+  o << lay.str() << xbase.str();
+  o << "  if (tid == 0u) {\n";
+  for (size_t gi = 0; gi < NG; ++gi) o << "    stg[" << gi << "] = R" << gi << ";\n";
+  for (size_t j = 0; j < nested.size(); ++j) o << "    stg[" << NG + j << "] = Q" << nested[j] << ";\n";
+  o << "  }\n";
+  for (size_t gi = 0; gi < NG; ++gi) {
+    const uint32_t s = group_scope(gi), AW = group_words(gi);
+    o << "  {   // exports of scope " << s << " (row loop " << gi << ")\n    const uint32_t* __restrict__ src = xs + X" << gi << " + (size_t)b" << s << " * " << AW << "u;\n"
+      << "    for (uint32_t i = tid; i < c" << s << " * " << AW << "u; i += nthr) GK_SPEC_CP4(stg + R" << gi << " + i, src + i);\n  }\n";
+  }
+  // the offsets of sibling scopes are read at the same parent rows: one item stages all of a parent's children (independent loads)
+  std::map<uint32_t, std::vector<uint32_t>> children;
+  for (uint32_t s : nested) children[parent_of(s)].push_back(s);
   for (auto& ch : children) {
     const uint32_t P = ch.first;
-    o << "    if (k <= c" << P << ") {   // offsets of the children of scope " << P << "\n";
-    for (uint32_t s : ch.second) o << "      const uint32_t x" << s << " = GK_SPEC_LD(scopes[" << s << "].off + b" << P << " + k);\n";
-    for (uint32_t s : ch.second) o << "      stg[Q" << s << " + k] = x" << s << " - b" << s << ";\n";
-    o << "      continue;\n    }\n    k -= c" << P << " + 1u;\n";
+    o << "  for (uint32_t k = tid; k <= c" << P << "; k += nthr) {   // offsets of the children of scope " << P << "\n";
+    for (uint32_t s : ch.second) o << "    const uint32_t x" << s << " = GK_SPEC_LD(scopes[" << s << "].off + b" << P << " + k);\n";
+    for (uint32_t s : ch.second) o << "    stg[Q" << s << " + k] = x" << s << " - b" << s << ";\n";
+    o << "  }\n";
   }
-  o << "  }\n}\n";
+  o << "  GK_SPEC_CP_WAIT();\n}\n";
   // ---- phase 2, gk_spec_object(): one thread per object, from shared memory.  Returns true when the object has more rows in some
   // scope than a mask holds: its words are then meaningless (the caller hands the tile to the interpreter, which stores them again;
   // a matcher error may be listed twice, with the same code).  `o` is the object's index in the tile, `obj` its index in the batch.
   o << "\nGK_SPEC_FN bool gk_spec_object(const GkBatch& B, const uint32_t* stg, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes,\n"
        "                               const uint32_t* actw, const GkOut& out, const uint32_t obj, const uint32_t o, uint32_t* vw, uint32_t* ew) {\n";
   o << "  const uint32_t lo0 = o, hi0 = o + 1u, n0 = 1u, f0 = 1u;\n  (void)lo0; (void)hi0; (void)n0; (void)f0; (void)out; (void)pool; (void)cbytes; (void)stg;\n";
-  o << "  const bool skip = (GK_SPEC_LD(B.flags + obj) & GK_F_SKIP) != 0u;\n  (void)skip;\n  bool big = false;\n";
+  o << "  bool big = false;\n";
   for (size_t j = 0; j < nested.size(); ++j) {
     const uint32_t s = nested[j], P = parent_of(s);
     o << "  const uint32_t* __restrict__ q" << s << " = stg + stg[" << NG + j << "];\n";

@@ -18,19 +18,23 @@
 namespace gk {
 
 struct SpecSource {
-  std::string src;        // one self-contained translation unit: program.h + vm_core.h + gk_spec_stage() + gk_spec_object() + gk_spec_kernel
+  std::string src;        // one self-contained translation unit: program.h + vm_core.h + gk_spec_row_<g>() + gk_spec_rows_kernel + gk_spec_stage()
+                          // + gk_spec_object() + gk_spec_kernel
   uint32_t words = 1;     // bitmap words per object
   size_t smem = 0;        // fixed dynamic shared memory of a launch (column / scope tables, enforcement-point mask, totals)
   size_t n_fast = 0, n_generic = 0;   // atoms emitted as immediates / as calls of the generic gk_atom()
-  // the per-tile staging area behind the fixed part: `hdr` words, then one region per entry of `stage`
+  // the per-tile staging area behind the fixed part: `hdr` words, then one region per entry of `stage` (the first `ngroups` are the
+  // row loops' exports, in row-loop order; the rest the nested scopes' offsets)
   struct StageRegion {
     uint32_t scope, per_row, extra;   // words = (rows of `scope` in the tile) * per_row + extra
   };
   std::vector<StageRegion> stage;
   uint32_t stage_hdr = 0;
-  // per scope with atoms: what phase 1 evaluates on a row (atoms, row-local gates) and what it stages of it (exports, by read form)
+  uint32_t ngroups = 0;
+  // per scope with atoms: what a row evaluates (atoms, row-local gates) and what it exports (by read form; on scope 0 the mask-form
+  // exports include the match and error bits of the spec.match blocks), in `words` words per row
   struct Fold {
-    uint32_t scope, atoms, gates, any, mask;
+    uint32_t scope, atoms, gates, any, mask, words;
   };
   std::vector<Fold> fold;
   // "folded: scope S: A atoms + G gates -> X any + Y mask in W words; ..." (the first line of `src`, and the backend's trace)
@@ -39,7 +43,7 @@ struct SpecSource {
     for (size_t i = 0; i < fold.size(); ++i) {
       const Fold& f = fold[i];
       t += std::string(i ? ";" : "") + " scope " + std::to_string(f.scope) + ": " + std::to_string(f.atoms) + " atoms + " + std::to_string(f.gates) + " gates -> " +
-           std::to_string(f.any) + " any + " + std::to_string(f.mask) + " mask in " + std::to_string(stage[i].per_row) + " words";
+           std::to_string(f.any) + " any + " + std::to_string(f.mask) + " mask in " + std::to_string(f.words) + " words";
     }
     return t;
   }
@@ -48,6 +52,18 @@ struct SpecSource {
     size_t w = stage_hdr;
     for (const StageRegion& r : stage) w += (size_t)(r.scope < cap.size() ? cap[r.scope] : 0u) * r.per_row + r.extra;
     return w * 4;
+  }
+  // bytes of the export arrays (gk_spec_rows_kernel -> gk_spec_kernel) of a batch with rows[s] rows in scope s (rows[0] = objects)
+  size_t export_bytes(const std::vector<uint32_t>& rows) const {
+    size_t w = 0;
+    for (uint32_t g = 0; g < ngroups; ++g) w += (size_t)(stage[g].scope < rows.size() ? rows[stage[g].scope] : 0u) * stage[g].per_row;
+    return w * 4;
+  }
+  // blocks of gk_spec_rows_kernel over such a batch at `threads` per block
+  uint32_t rows_blocks(const std::vector<uint32_t>& rows, uint32_t threads) const {
+    uint64_t b = 0;
+    for (uint32_t g = 0; g < ngroups; ++g) b += ((stage[g].scope < rows.size() ? rows[stage[g].scope] : 0u) + (uint64_t)threads - 1) / threads;
+    return (uint32_t)b;
   }
 };
 

@@ -1,8 +1,11 @@
-"""GPU probe: the kernel generated for the constraint set (gk_spec_kernel, NVRTC) against the netlist interpreter
-(gk_eval_kernel) on a resident page of a BASELINE configuration -- identical bitmaps / totals, and the launch time of
-several build variants (threads per CTA x minimum resident CTAs = register cap).
+"""GPU probe: the kernels generated for the constraint set (gk_spec_rows_kernel + gk_spec_kernel, NVRTC) against the netlist
+interpreter (gk_eval_kernel) on a resident page of a BASELINE configuration -- identical bitmaps / totals / error lists, and the
+launch time (both kernels) of several build variants (threads per CTA x minimum resident CTAs = register cap).
 
-    python tools/spec_probe.py [--config 2] [--objects 1000000] [--variants 512x1,512x1:GENERIC,256x2,384x1,512x1:NOMATCH]
+    python tools/spec_probe.py [--config 2] [--objects 1000000] [--variants 256x3,256x3@256x8,256x2,256x3:NOMATCH,256x3:STAGEONLY]
+
+A variant is TILExMINB[@ROWSxMINB][:SWITCH+SWITCH]: the shape of gk_spec_kernel, optionally of gk_spec_rows_kernel, and measurement
+switches of the text (GENERIC = spec.match through the shared gk_match(); otherwise -DGK_SPEC_X_<SWITCH>: NOMATCH, STAGEONLY).
 """
 import argparse
 import json
@@ -18,7 +21,7 @@ sys.path.insert(0, ROOT)
 ap = argparse.ArgumentParser()
 ap.add_argument("--config", type=int, default=2)
 ap.add_argument("--objects", type=int, default=1000000)
-ap.add_argument("--variants", default="512x1,512x1:GENERIC,256x2,384x1,512x1:NOMATCH")
+ap.add_argument("--variants", default="256x3,256x3@256x8,256x2,256x3:NOMATCH,256x3:STAGEONLY")
 ap.add_argument("--steps", type=int, default=10)
 ap.add_argument("--wide", type=int, default=0, help="every WIDE-th object gets 40 containers (exercises the tile hand-over)")
 a = ap.parse_args()
@@ -56,7 +59,7 @@ if a.wide:
 
 
 def run(label, env):
-    for k in ("GK_SPEC", "GK_SPEC_THREADS", "GK_SPEC_MINB", "GK_SPEC_DEFS"):
+    for k in ("GK_SPEC", "GK_SPEC_THREADS", "GK_SPEC_MINB", "GK_SPEC_ROWS_THREADS", "GK_SPEC_ROWS_MINB", "GK_SPEC_DEFS"):
         os.environ.pop(k, None)
     os.environ.update(env)
     drv = engine()
@@ -72,7 +75,7 @@ def run(label, env):
     out = {"label": label, "kernel": drv.last_kernel(), "kernel_ms": round(sum(ms) / len(ms), 4), "min_ms": round(min(ms), 4), "first_eval_s": round(first_s, 2),
            "alg_bytes": rb.alg_bytes + a.objects * r.viol_bits.shape[1] * 8}
     out["GBps"] = round(out["alg_bytes"] / out["kernel_ms"] / 1e6, 1)
-    res = (np.array(r.viol_bits, copy=True), np.array(r.err_bits, copy=True), list(r.totals), list(r.err_totals))
+    res = (np.array(r.viol_bits, copy=True), np.array(r.err_bits, copy=True), list(r.totals), list(r.err_totals), sorted((x.object, x.constraint, x.msg) for x in r.results if x.autoreject))
     rb.free()
     drv.pin_blob(blob, False)
     drv.close()
@@ -81,14 +84,16 @@ def run(label, env):
 
 base, want = run("interpreter", {"GK_SPEC": "0"})
 print(json.dumps(base), flush=True)
-for v in a.variants.split(","):     # THREADSxMINB[:SWITCH+SWITCH]: GENERIC = spec.match through the shared gk_match(); NOMATCH = -DGK_SPEC_X_NOMATCH (results differ)
+for v in a.variants.split(","):
     v, _, sw = v.partition(":")
+    v, _, rv = v.partition("@")
     th, mb = v.split("x")
+    rows = dict(zip(("GK_SPEC_ROWS_THREADS", "GK_SPEC_ROWS_MINB"), rv.split("x"))) if rv else {}
     toks = [x for x in sw.split("+") if x]
     defs = " ".join("-DGK_SPEC_X_" + x for x in toks if x != "GENERIC")
     os.environ["GK_SPEC_MATCHGEN"] = "0" if "GENERIC" in toks else "1"
-    o, got = run("spec " + v + (" " + sw if sw else ""), {"GK_SPEC_THREADS": th, "GK_SPEC_MINB": mb, "GK_SPEC_MIN_OBJECTS": "0", "GK_SPEC_DEFS": defs})
-    o["identical"] = bool(np.array_equal(want[0], got[0]) and np.array_equal(want[1], got[1]) and want[2] == got[2] and want[3] == got[3])
+    o, got = run("spec " + v + ("@" + rv if rv else "") + (" " + sw if sw else ""), dict(rows, GK_SPEC_THREADS=th, GK_SPEC_MINB=mb, GK_SPEC_MIN_OBJECTS="0", GK_SPEC_DEFS=defs))
+    o["identical"] = bool(np.array_equal(want[0], got[0]) and np.array_equal(want[1], got[1]) and want[2:] == got[2:])
     print(json.dumps(o), flush=True)
-    assert o["identical"] or "NOMATCH" in sw, "generated kernel and interpreter disagree"
+    assert o["identical"] or "NOMATCH" in sw or "STAGEONLY" in sw, "generated kernel and interpreter disagree"
     assert o["kernel"] == "gk_spec_kernel" or "hostemu" in os.environ.get("GK_ENGINE_LIB", ""), "the generated kernel did not run"
