@@ -2,10 +2,10 @@
 #include <chrono>
 #include <condition_variable>
 #include <deque>
+#include <exception>
 #include <mutex>
 #include <cstdlib>
 #include <cstring>
-#include <functional>
 #include <memory>
 #include <stdexcept>
 #include <thread>
@@ -113,10 +113,28 @@ struct ProgramLease {
   ProgramLease(const ProgramLease&) = delete;
   ProgramLease& operator=(const ProgramLease&) = delete;
 };
+
+// Releases a backend handle -- a device batch or a kept page source -- when its owner dies.  No exception leaves it: it runs in
+// destructors.
+struct BackendRelease {
+  Backend* be = nullptr;
+  void (Backend::*call)(void*) = nullptr;
+  void operator()(void* p) const noexcept {
+    try {
+      (be->*call)(p);
+    } catch (...) {
+    }
+  }
+};
+using BackendHandle = std::unique_ptr<void, BackendRelease>;
+
+BackendHandle device_batch(gk_engine* e, void* dev) { return BackendHandle(dev, BackendRelease{e->be.get(), &Backend::release}); }
+BackendHandle kept_source(gk_engine* e, void* source) { return BackendHandle(source, BackendRelease{e->be.get(), &Backend::release_source}); }
 }  // namespace
 
+// A resident batch.  It owns its device batch and its kept source: both are released with it, through the backend that made them.
 struct gk_batch {
-  void* dev = nullptr;
+  BackendHandle dev;
   std::shared_ptr<const Compiled> compiled;
   std::shared_ptr<HostBatch> host;     // kept for object_errors / alg_bytes (column data is released after upload)
   std::vector<gk_obj> objs;            // shallow copy: the caller keeps the JSON alive while the batch lives
@@ -131,7 +149,7 @@ struct gk_batch {
   std::vector<std::string> excluded;   // the excluder patterns of the upload's process the batch was flattened with
   // GK_F_KEEP_SOURCE: the page's source (Backend::ingest_keep -- on the GPU its device JSON, offsets and token tape), and the
   // review-level errors of its objects (they depend on the page alone)
-  void* source = nullptr;
+  BackendHandle source;
   std::vector<std::string> source_errors;
   ObjIn obj_in(size_t i) const;
 };
@@ -255,7 +273,7 @@ void eval_batch(gk_engine* e, gk_batch* b, const char* ep_c, uint32_t flags, gk_
   e->eng->active_mask(c, ep, active);
   bool copy_back = !(flags & GK_F_NO_COPY_BACK) || (flags & GK_F_MATERIALIZE);
   double t0 = now_ms();
-  e->be->eval(b->dev, active, rp->ev, copy_back);
+  e->be->eval(b->dev.get(), active, rp->ev, copy_back);
   double t1 = now_ms();
   rp->obj_errors = b->host->obj_errors;
   out->d2h_bytes = copy_back ? (uint64_t)rp->ev.viol.size() * 8 : 0;
@@ -329,8 +347,38 @@ std::vector<std::string> excluded_of(gk_engine* e, uint32_t flags) {
   return process.empty() ? std::vector<std::string>() : e->eng->excluded_namespaces(process);
 }
 
-void upload_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, const gk_obj* objs, size_t n, uint32_t flags, gk_batch** outb,
-                  gk_result* stats) {
+// A resident batch of `n` objects flattened against `c` onto the device batch `dev`: the fields every upload fills, and its
+// statistics.  `errors`: the objects' review-level errors (empty: none).
+std::unique_ptr<gk_batch> make_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, BackendHandle dev, uint32_t n, uint32_t flags,
+                                     std::vector<std::string> errors, std::vector<std::string> excluded, const IngestStats& ist, double flatten_ms,
+                                     gk_result* stats) {
+  auto b = std::make_unique<gk_batch>();
+  b->dev = std::move(dev);
+  b->compiled = c;
+  if (c->uses_data) e->eng->data_doc(&b->data_version);
+  b->n = n;
+  b->flags = flags;
+  b->alg_bytes = ist.alg_bytes;
+  b->excluded = std::move(excluded);
+  // the host column data is not kept; the small per-object error list is
+  auto slim = std::make_shared<HostBatch>();
+  slim->n = n;
+  slim->obj_errors = std::move(errors);
+  slim->alg_bytes = ist.alg_bytes;
+  b->host = slim;
+  if (stats) {
+    stats->flatten_ms = flatten_ms;
+    stats->h2d_ms = ist.h2d_ms;
+    stats->h2d_bytes = ist.h2d_bytes;
+    stats->alg_bytes = ist.alg_bytes;
+    stats->n_objects = n;
+    stats->n_constraints = (uint32_t)c->cons_match.size();
+  }
+  return b;
+}
+
+std::unique_ptr<gk_batch> upload_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, const gk_obj* objs, size_t n, uint32_t flags,
+                                       gk_result* stats) {
   std::vector<std::string> excluded = excluded_of(e, flags);   // (read before the flatten: a later change makes the batch stale, never current)
   std::vector<ObjIn> ins(n);
   for (size_t i = 0; i < n; ++i) ins[i] = to_in(objs[i]);
@@ -338,32 +386,14 @@ void upload_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, const 
   auto hb = e->eng->flatten(ins.data(), n, *c, process_of(flags));
   double t1 = now_ms();
   e->be->sync_strings(e->eng->strings());
-  auto b = std::make_unique<gk_batch>();
-  double h2d_ms = 0;
+  IngestStats ist;
   uint64_t h2d_bytes = 0;
-  b->dev = e->be->upload(*hb, *c, &h2d_ms, &h2d_bytes);
-  b->compiled = c;
-  if (c->uses_data) e->eng->data_doc(&b->data_version);
-  b->n = hb->n;
-  b->flags = flags;
-  b->alg_bytes = hb->alg_bytes;
-  b->excluded = std::move(excluded);
+  BackendHandle dev = device_batch(e, e->be->upload(*hb, *c, &ist.h2d_ms, &h2d_bytes));
+  ist.h2d_bytes = h2d_bytes;
+  ist.alg_bytes = hb->alg_bytes;
+  auto b = make_batch(e, c, std::move(dev), hb->n, flags, std::move(hb->obj_errors), std::move(excluded), ist, t1 - t0, stats);
   b->objs.assign(objs, objs + n);
-  // drop the host column data; keep the small per-object error list
-  auto slim = std::make_shared<HostBatch>();
-  slim->n = hb->n;
-  slim->obj_errors = std::move(hb->obj_errors);
-  slim->alg_bytes = hb->alg_bytes;
-  b->host = slim;
-  if (stats) {
-    stats->flatten_ms = t1 - t0;
-    stats->h2d_ms = h2d_ms;
-    stats->h2d_bytes = h2d_bytes;
-    stats->alg_bytes = hb->alg_bytes;
-    stats->n_objects = hb->n;
-    stats->n_constraints = (uint32_t)c->cons_match.size();
-  }
-  *outb = b.release();
+  return b;
 }
 
 static std::vector<gk_obj> blob_objs(const char* buf, const uint64_t* off, size_t n, uint8_t source) {
@@ -382,88 +412,161 @@ bool device_ingest(const Compiled& c, size_t n) {
   return c.device_ingest && !host_only && n != 0 && !getenv("GK_NO_DEVICE_INGEST_RUNTIME");   // (the runtime switch is for A/B tests)
 }
 
-// A batch ingested on the device, or re-extracted from its kept source (`ist`, `t0`: the ingest's statistics and start); the
-// review-level errors of its objects are `errors` (empty: none).
-std::unique_ptr<gk_batch> blob_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, void* dev, const char* buf, const uint64_t* off, size_t n,
-                                     uint8_t source, uint32_t flags, std::vector<std::string> errors, const IngestStats& ist, double t0, gk_result* stats) {
-  auto b = std::make_unique<gk_batch>();
-  b->dev = dev;
-  b->compiled = c;
-  if (c->uses_data) e->eng->data_doc(&b->data_version);
-  b->n = (uint32_t)n;
-  b->flags = flags;
-  b->alg_bytes = ist.alg_bytes;
+// a blob of plain objects: flattened by the ingest kernels on the device when the compiled snapshot allows it
+std::unique_ptr<gk_batch> upload_blob(gk_engine* e, const std::shared_ptr<const Compiled>& c, const char* buf, const uint64_t* off, size_t n, uint8_t source,
+                                      uint32_t flags, gk_result* stats) {
+  std::unique_ptr<gk_batch> b;
+  if (!device_ingest(*c, n)) {
+    auto v = blob_objs(buf, off, n, source);
+    b = upload_batch(e, c, v.data(), n, flags, stats);   // (kept as a blob too: a later gk_batch_refresh may ingest it on the device)
+  } else {
+    double t0 = now_ms();
+    IngestReq rq = e->eng->ingest_request(c, reinterpret_cast<const uint8_t*>(buf), reinterpret_cast<const unsigned long long*>(off), n, source, process_of(flags));
+    IngestStats ist;
+    std::vector<uint32_t> status;
+    void* kept = nullptr;
+    BackendHandle dev = device_batch(e, (flags & GK_F_KEEP_SOURCE) ? e->be->ingest_keep(rq, &ist, &status, &kept) : e->be->ingest(rq, &ist, &status));
+    BackendHandle source_kept = kept_source(e, kept);
+    std::vector<std::string> errors;
+    for (size_t i = 0; i < n; ++i)
+      if (status[i] != GK_ING_OK) {
+        if (errors.empty()) errors.assign(n, std::string());   // (left empty when every object is fine)
+        // the rare rejected object: the host parser words the review-level error (bad JSON, not an object, kind missing)
+        ObjIn in;
+        in.json = buf + off[i];
+        in.len = (size_t)(off[i + 1] - off[i]);
+        in.source = source;
+        std::string err;
+        VP doc = e->eng->review_doc(in, nullptr, nullptr, nullptr, &err);
+        if (doc && status[i] != GK_ING_NULL) err = "device ingest refused the object (status " + std::to_string(status[i]) + "): JSON nesting deeper than " +
+                                                 std::to_string(GK_TAPE_MAX_DEPTH) + " levels or a token longer than 128 MiB";
+        if (!doc && err.empty()) err = "invalid request object";
+        errors[i] = err;
+      }
+    b = make_batch(e, c, std::move(dev), (uint32_t)n, flags, errors, std::move(rq.excluded), ist, (now_ms() - t0) - ist.h2d_ms, stats);
+    if (source_kept) {
+      b->source = std::move(source_kept);
+      b->source_errors = std::move(errors);
+    }
+  }
   b->blob = buf;
   b->blob_off = off;
   b->blob_source = source;
-  auto slim = std::make_shared<HostBatch>();
-  slim->n = (uint32_t)n;
-  slim->alg_bytes = ist.alg_bytes;
-  slim->obj_errors = std::move(errors);
-  b->host = slim;
-  if (stats) {
-    stats->flatten_ms = (now_ms() - t0) - ist.h2d_ms;
-    stats->h2d_ms = ist.h2d_ms;
-    stats->h2d_bytes = ist.h2d_bytes;
-    stats->alg_bytes = ist.alg_bytes;
-    stats->n_objects = (uint32_t)n;
-    stats->n_constraints = (uint32_t)c->cons_match.size();
-  }
   return b;
-}
-
-// a blob of plain objects: flattened by the ingest kernels on the device when the compiled snapshot allows it
-void upload_blob(gk_engine* e, const std::shared_ptr<const Compiled>& c, const char* buf, const uint64_t* off, size_t n, uint8_t source, uint32_t flags,
-                 gk_batch** outb, gk_result* stats) {
-  if (!device_ingest(*c, n)) {
-    auto v = blob_objs(buf, off, n, source);
-    upload_batch(e, c, v.data(), n, flags, outb, stats);
-    (*outb)->blob = buf;   // (the objects of `objs`, as a blob: a later gk_batch_refresh may ingest them on the device)
-    (*outb)->blob_off = off;
-    (*outb)->blob_source = source;
-    return;
-  }
-  double t0 = now_ms();
-  IngestReq rq = e->eng->ingest_request(c, reinterpret_cast<const uint8_t*>(buf), reinterpret_cast<const unsigned long long*>(off), n, source, process_of(flags));
-  IngestStats ist;
-  std::vector<uint32_t> status;
-  void* kept = nullptr;
-  void* dev = (flags & GK_F_KEEP_SOURCE) ? e->be->ingest_keep(rq, &ist, &status, &kept) : e->be->ingest(rq, &ist, &status);
-  std::vector<std::string> errors;
-  for (size_t i = 0; i < n; ++i)
-    if (status[i] != GK_ING_OK) {
-      if (errors.empty()) errors.assign(n, std::string());   // (left empty when every object is fine)
-      // the rare rejected object: the host parser words the review-level error (bad JSON, not an object, kind missing)
-      ObjIn in;
-      in.json = buf + off[i];
-      in.len = (size_t)(off[i + 1] - off[i]);
-      in.source = source;
-      std::string err;
-      VP doc = e->eng->review_doc(in, nullptr, nullptr, nullptr, &err);
-      if (doc && status[i] != GK_ING_NULL) err = "device ingest refused the object (status " + std::to_string(status[i]) + "): JSON nesting deeper than " +
-                                               std::to_string(GK_TAPE_MAX_DEPTH) + " levels or a token longer than 128 MiB";
-      if (!doc && err.empty()) err = "invalid request object";
-      errors[i] = err;
-    }
-  auto b = blob_batch(e, c, dev, buf, off, n, source, flags, errors, ist, t0, stats);
-  b->excluded = rq.excluded;
-  if (kept) {
-    b->source = kept;
-    b->source_errors = std::move(errors);
-  }
-  *outb = b.release();
 }
 
 // gk_batch_refresh of a batch that kept its source, for a snapshot flattened on the device: the extraction passes again, from the
 // page's token tape in HBM -- no copy, no tokeniser, and the caller's blob is not read
-void refresh_from_source(gk_engine* e, const std::shared_ptr<const Compiled>& c, const gk_batch* old, gk_batch** outb, gk_result* stats) {
+std::unique_ptr<gk_batch> refresh_from_source(gk_engine* e, const std::shared_ptr<const Compiled>& c, const gk_batch& old, gk_result* stats) {
   double t0 = now_ms();
-  IngestReq rq = e->eng->ingest_request(c, nullptr, nullptr, old->n, old->blob_source, process_of(old->flags));
+  IngestReq rq = e->eng->ingest_request(c, nullptr, nullptr, old.n, old.blob_source, process_of(old.flags));
   IngestStats ist;
-  void* dev = e->be->reextract(old->source, rq, &ist);
-  auto b = blob_batch(e, c, dev, old->blob, old->blob_off, old->n, old->blob_source, old->flags, old->source_errors, ist, t0, stats);
-  b->excluded = rq.excluded;
-  *outb = b.release();
+  BackendHandle dev = device_batch(e, e->be->reextract(old.source.get(), rq, &ist));
+  auto b = make_batch(e, c, std::move(dev), old.n, old.flags, old.source_errors, std::move(rq.excluded), ist, (now_ms() - t0) - ist.h2d_ms, stats);
+  b->blob = old.blob;
+  b->blob_off = old.blob_off;
+  b->blob_source = old.blob_source;
+  return b;
+}
+
+// the bitmap-only calls: they would leave out the resultants of generator objects, silently
+void refuse_while_expanding(gk_engine* e) {
+  if (e->eng->has_expansion())
+    throw RegoError{"ExpansionTemplates are registered: this entry point does not expand generator objects -- review them through gk_review_batch, or "
+                    "aggregate the batch with gk_audit_add_batch, which do"};
+}
+
+// why batch `b` is stale against snapshot `c` (null: it is current)
+const char* stale_reason(gk_engine* e, const Compiled& c, const gk_batch& b) {
+  if (c.version != b.compiled->version) return "batch was flattened against an older constraint set; upload it again";
+  if (c.uses_data) {   // the columns of a referential snapshot hold values computed from data.inventory
+    uint64_t dv = 0;
+    e->eng->data_doc(&dv);
+    if (dv != b.data_version) return "data.inventory changed since the batch was flattened (referential constraints); upload it again";
+  }
+  return nullptr;
+}
+
+void require_current(gk_engine* e, const Compiled& c, const gk_batch& b) {
+  if (const char* why = stale_reason(e, c, b)) throw RegoError{why};
+}
+
+// gk_batch_eval_device and gk_batch_eval_device_peers: the kernel's outputs go to the caller's device buffers `d`
+void eval_device(gk_engine* e, const gk_batch& b, const char* ep, const DevOutPtrs& d) {
+  refuse_while_expanding(e);
+  auto c = e->eng->compiled();
+  require_current(e, *c, b);
+  ProgramLease lease(e, *c);
+  std::vector<uint32_t> active;
+  e->eng->active_mask(*c, ep ? ep : "", active);
+  e->be->eval_into(b.dev.get(), active, d);
+}
+
+// ---- expansion (pkg/audit/manager.go:733-765, pkg/webhook/policy.go:610-646), the step gk_review_batch and the audit share: the
+// resultants of generator objects are reviewed as generated resources, and their results folded back onto their parents
+struct Child {
+  uint32_t parent;
+  std::string json, tmpl, action;
+};
+
+struct Expansion {
+  std::vector<Child> children;       // in object order
+  std::vector<std::string> errors;   // per object: "" or why its expansion failed
+};
+
+// Expands every object of `ins` but those with a non-empty skip[i] (`skip` may be empty); a large page is spread over the host threads.
+Expansion expand_page(Engine& eng, const std::vector<ObjIn>& ins, const std::vector<std::string>& skip, int threads) {
+  const size_t n = ins.size();
+  const size_t T = std::min<size_t>((size_t)std::max(1, threads), std::max<size_t>(1, n / 256));
+  Expansion x;
+  x.errors.assign(n, std::string());
+  std::vector<std::vector<Child>> part(T);
+  std::vector<std::exception_ptr> failed(T);
+  auto work = [&](size_t t) {
+    try {
+      std::vector<Resultant> res;
+      for (size_t i = n * t / T; i < n * (t + 1) / T; ++i) {
+        if (i < skip.size() && !skip[i].empty()) continue;
+        res.clear();
+        try {
+          eng.expand_object(ins[i], res);
+        } catch (std::runtime_error& e) {   // (System.Expand's errors)
+          x.errors[i] = std::string("unable to expand object: ") + e.what();
+          continue;
+        }
+        for (auto& r : res) part[t].push_back(Child{(uint32_t)i, json_str(r.obj), r.template_name, r.action});
+      }
+    } catch (...) {
+      failed[t] = std::current_exception();
+    }
+  };
+  if (T == 1) work(0);
+  else {
+    std::vector<std::thread> th;
+    for (size_t t = 0; t < T; ++t) th.emplace_back(work, t);
+    for (auto& h : th) h.join();
+  }
+  for (auto& f : failed)
+    if (f) std::rethrow_exception(f);
+  for (auto& p : part) x.children.insert(x.children.end(), std::make_move_iterator(p.begin()), std::make_move_iterator(p.end()));
+  return x;
+}
+
+// the resultants as review objects: the parent's Namespace (createReviewForResultant), source Generated
+std::vector<gk_obj> resultant_objs(const std::vector<Child>& children, const std::vector<ObjIn>& parents) {
+  std::vector<gk_obj> v(children.size());
+  for (size_t k = 0; k < children.size(); ++k) {
+    gk_obj& o = v[k];
+    memset(&o, 0, sizeof o);
+    o.json = children[k].json.data();
+    o.len = children[k].json.size();
+    const ObjIn& par = parents[children[k].parent];
+    o.ns_json = par.ns_json;
+    o.ns_len = par.ns_len;
+    o.ns_name = par.ns_name;
+    o.source = GK_SOURCE_GENERATED;
+  }
+  return v;
 }
 
 }  // namespace
@@ -600,63 +703,32 @@ int gk_review_batch(gk_engine_t* e, const gk_obj* objs, size_t n, const char* ep
   if (!e || !out || (!objs && n)) return GK_ERR_INVALID;
   memset(out, 0, sizeof *out);
   return guard(err, [&]() {
-    // ---- expansion (pkg/audit/manager.go:733-765, pkg/webhook/policy.go:610-646): the resultants of generator objects are
-    // appended to the batch as generated resources, reviewed with it, and their results folded back onto their parents
-    struct Child {
-      uint32_t parent;
-      std::string json, tmpl, action;
-    };
-    std::vector<Child> children;
-    std::vector<std::string> expand_errors;
+    // ---- expansion: the resultants are appended to the batch, reviewed with it, and folded back below
+    Expansion x;
+    std::vector<gk_obj> all;   // (empty: the objects alone)
     if (e->eng->has_expansion()) {
-      expand_errors.assign(n, std::string());
-      std::vector<Resultant> res;
-      for (size_t i = 0; i < n; ++i) {
-        res.clear();
-        try {
-          e->eng->expand_object(to_in(objs[i]), res);
-        } catch (std::runtime_error& x) {
-          expand_errors[i] = std::string("unable to expand object: ") + x.what();
-          continue;
-        }
-        for (auto& r : res) children.push_back(Child{(uint32_t)i, json_str(r.obj), r.template_name, r.action});
+      std::vector<ObjIn> ins(n);
+      for (size_t i = 0; i < n; ++i) ins[i] = to_in(objs[i]);
+      x = expand_page(*e->eng, ins, {}, e->eng->threads());
+      if (!x.children.empty()) {
+        all.assign(objs, objs + n);
+        const std::vector<gk_obj> res = resultant_objs(x.children, ins);
+        all.insert(all.end(), res.begin(), res.end());
       }
     }
-    std::vector<gk_obj> all;
-    const gk_obj* use = objs;
-    size_t total = n;
-    if (!children.empty()) {
-      all.assign(objs, objs + n);
-      for (auto& c : children) {
-        gk_obj o;
-        memset(&o, 0, sizeof o);
-        o.json = c.json.data();
-        o.len = c.json.size();
-        o.ns_json = objs[c.parent].ns_json;       // createReviewForResultant: the parent's Namespace, source Generated
-        o.ns_len = objs[c.parent].ns_len;
-        o.ns_name = objs[c.parent].ns_name;
-        o.source = GK_SOURCE_GENERATED;
-        all.push_back(o);
-      }
-      use = all.data();
-      total = all.size();
-    }
-    gk_batch* b = nullptr;
+    const gk_obj* use = all.empty() ? objs : all.data();
+    const size_t total = all.empty() ? n : all.size();
     gk_result stats;
     memset(&stats, 0, sizeof stats);
     auto c = e->eng->compiled();
     ProgramLease lease(e, *c);   // flatten + upload + kernel + rendering all against this one snapshot
-    upload_batch(e, c, use, total, flags, &b, &stats);
-    std::unique_ptr<gk_batch, std::function<void(gk_batch*)>> hold(b, [&](gk_batch* x) {
-      e->be->release(x->dev);
-      delete x;
-    });
-    eval_batch(e, b, ep, flags, out);
+    auto b = upload_batch(e, c, use, total, flags, &stats);
+    eval_batch(e, b.get(), ep, flags, out);
     out->flatten_ms = stats.flatten_ms;
     out->h2d_ms = stats.h2d_ms;
     out->h2d_bytes = stats.h2d_bytes;
-    bool any_expand_err = false;
-    for (auto& x : expand_errors) any_expand_err = any_expand_err || !x.empty();
+    const std::vector<Child>& children = x.children;
+    const bool any_expand_err = std::any_of(x.errors.begin(), x.errors.end(), [](const std::string& m) { return !m.empty(); });
     if (children.empty() && !any_expand_err) return;
     // ---- fold the resultants back: bits ORed into the parent's row, results re-indexed with "[Implied by <template>]" and the
     // template's enforcement-action override (aggregate.go:19-63), their review-level errors reported on the parent
@@ -686,8 +758,8 @@ int gk_review_batch(gk_engine_t* e, const gk_obj* objs, size_t n, const char* ep
         if (!rp->obj_errors[n + k].empty() && rp->obj_errors[children[k].parent].empty())
           rp->obj_errors[children[k].parent] = ExpansionSystem::implied_by(children[k].tmpl, rp->obj_errors[n + k]);
       rp->obj_errors.resize(n);
-      for (size_t i = 0; i < n && i < expand_errors.size(); ++i)
-        if (!expand_errors[i].empty() && rp->obj_errors[i].empty()) rp->obj_errors[i] = expand_errors[i];
+      for (size_t i = 0; i < n && i < x.errors.size(); ++i)
+        if (!x.errors[i].empty() && rp->obj_errors[i].empty()) rp->obj_errors[i] = x.errors[i];
     }
     const bool give_bits = !(flags & GK_F_NO_COPY_BACK);
     fill_result(out, rp, give_bits);
@@ -700,7 +772,7 @@ int gk_batch_upload(gk_engine_t* e, const gk_obj* objs, size_t n, uint32_t flags
   return guard(err, [&]() {
     auto c = e->eng->compiled();
     ProgramLease lease(e, *c);
-    upload_batch(e, c, objs, n, flags, outb, stats);
+    *outb = upload_batch(e, c, objs, n, flags, stats).release();
   });
 }
 
@@ -708,16 +780,9 @@ int gk_batch_eval(gk_engine_t* e, gk_batch_t* b, const char* ep, uint32_t flags,
   if (!e || !b || !out) return GK_ERR_INVALID;
   memset(out, 0, sizeof *out);
   return guard(err, [&]() {
-    if (e->eng->has_expansion())   // (bitmaps of the listed objects only: the resultants of generators would be missing, silently)
-      throw RegoError{"ExpansionTemplates are registered: this entry point does not expand generator objects -- review them through gk_review_batch, or "
-                      "aggregate the batch with gk_audit_add_batch, which do"};
+    refuse_while_expanding(e);
     auto c = e->eng->compiled();
-    if (c->version != b->compiled->version) throw RegoError{"batch was flattened against an older constraint set; upload it again"};
-    if (c->uses_data) {   // the columns of a referential snapshot hold values computed from data.inventory
-      uint64_t dv = 0;
-      e->eng->data_doc(&dv);
-      if (dv != b->data_version) throw RegoError{"data.inventory changed since the batch was flattened (referential constraints); upload it again"};
-    }
+    require_current(e, *c, *b);
     ProgramLease lease(e, *c);
     eval_batch(e, b, ep, flags, out);
   });
@@ -726,62 +791,31 @@ int gk_batch_eval(gk_engine_t* e, gk_batch_t* b, const char* ep, uint32_t flags,
 int gk_batch_eval_device(gk_engine_t* e, gk_batch_t* b, const char* ep, void* d_viol, void* d_err, void* d_totals, void* d_err_totals,
                          void* stream, char** err) {
   if (!e || !b || !d_viol || !d_err || !d_totals || !d_err_totals) return GK_ERR_INVALID;
-  return guard(err, [&]() {
-    if (e->eng->has_expansion())   // (bitmaps of the listed objects only: the resultants of generators would be missing, silently)
-      throw RegoError{"ExpansionTemplates are registered: this entry point does not expand generator objects -- review them through gk_review_batch, or "
-                      "aggregate the batch with gk_audit_add_batch, which do"};
-    auto c = e->eng->compiled();
-    if (c->version != b->compiled->version) throw RegoError{"batch was flattened against an older constraint set; upload it again"};
-    if (c->uses_data) {   // the columns of a referential snapshot hold values computed from data.inventory
-      uint64_t dv = 0;
-      e->eng->data_doc(&dv);
-      if (dv != b->data_version) throw RegoError{"data.inventory changed since the batch was flattened (referential constraints); upload it again"};
-    }
-    ProgramLease lease(e, *c);
-    std::vector<uint32_t> active;
-    e->eng->active_mask(*c, ep ? ep : "", active);
-    DevOutPtrs d;
-    d.viol = d_viol;
-    d.err = d_err;
-    d.totals = d_totals;
-    d.err_totals = d_err_totals;
-    d.stream = stream;
-    e->be->eval_into(b->dev, active, d);
-  });
+  DevOutPtrs d;
+  d.viol = d_viol;
+  d.err = d_err;
+  d.totals = d_totals;
+  d.err_totals = d_err_totals;
+  d.stream = stream;
+  return guard(err, [&]() { eval_device(e, *b, ep, d); });
 }
 
 int gk_batch_eval_device_peers(gk_engine_t* e, gk_batch_t* b, const char* ep, const uint64_t* peer_bases, uint32_t npeers, uint32_t rank,
                                uint64_t slot_i32, uint64_t tot_off_i32, uint32_t tot_stride, void* d_err, void* d_totals, void* d_err_totals,
                                void* stream, char** err) {
   if (!e || !b || !peer_bases || !npeers || npeers > 8 || rank >= npeers || !d_err || !d_totals || !d_err_totals) return GK_ERR_INVALID;
-  return guard(err, [&]() {
-    if (e->eng->has_expansion())   // (bitmaps of the listed objects only: the resultants of generators would be missing, silently)
-      throw RegoError{"ExpansionTemplates are registered: this entry point does not expand generator objects -- review them through gk_review_batch, or "
-                      "aggregate the batch with gk_audit_add_batch, which do"};
-    auto c = e->eng->compiled();
-    if (c->version != b->compiled->version) throw RegoError{"batch was flattened against an older constraint set; upload it again"};
-    if (c->uses_data) {   // the columns of a referential snapshot hold values computed from data.inventory
-      uint64_t dv = 0;
-      e->eng->data_doc(&dv);
-      if (dv != b->data_version) throw RegoError{"data.inventory changed since the batch was flattened (referential constraints); upload it again"};
-    }
-    ProgramLease lease(e, *c);
-    std::vector<uint32_t> active;
-    e->eng->active_mask(*c, ep ? ep : "", active);
-    DevOutPtrs d;
-    d.viol = nullptr;
-    d.err = d_err;
-    d.totals = d_totals;
-    d.err_totals = d_err_totals;
-    d.stream = stream;
-    d.npeers = npeers;
-    d.tot_stride = tot_stride;
-    for (uint32_t q = 0; q < npeers; ++q) {
-      d.peer_viol[q] = peer_bases[q] + (uint64_t)rank * slot_i32 * 4;
-      d.peer_tot[q] = peer_bases[q] + ((uint64_t)rank * slot_i32 + tot_off_i32) * 4;
-    }
-    e->be->eval_into(b->dev, active, d);
-  });
+  DevOutPtrs d;
+  d.err = d_err;
+  d.totals = d_totals;
+  d.err_totals = d_err_totals;
+  d.stream = stream;
+  d.npeers = npeers;
+  d.tot_stride = tot_stride;
+  for (uint32_t q = 0; q < npeers; ++q) {
+    d.peer_viol[q] = peer_bases[q] + (uint64_t)rank * slot_i32 * 4;
+    d.peer_tot[q] = peer_bases[q] + ((uint64_t)rank * slot_i32 + tot_off_i32) * 4;
+  }
+  return guard(err, [&]() { eval_device(e, *b, ep, d); });
 }
 
 int gk_batch_upload_blob(gk_engine_t* e, const char* buf, const uint64_t* offsets, size_t n, uint8_t source, uint32_t flags, gk_batch_t** outb,
@@ -791,7 +825,7 @@ int gk_batch_upload_blob(gk_engine_t* e, const char* buf, const uint64_t* offset
   return guard(err, [&]() {
     auto c = e->eng->compiled();
     ProgramLease lease(e, *c);
-    upload_blob(e, c, buf, offsets, n, source, flags, outb, stats);
+    *outb = upload_blob(e, c, buf, offsets, n, source, flags, stats).release();
   });
 }
 
@@ -800,20 +834,13 @@ int gk_review_blob(gk_engine_t* e, const char* buf, const uint64_t* offsets, siz
   if (!e || !out || ((!buf || !offsets) && n)) return GK_ERR_INVALID;
   memset(out, 0, sizeof *out);
   return guard(err, [&]() {
-    gk_batch* b = nullptr;
+    refuse_while_expanding(e);
     gk_result stats;
     memset(&stats, 0, sizeof stats);
-    if (e->eng->has_expansion())   // (bitmaps of the listed objects only: the resultants of generators would be missing, silently)
-      throw RegoError{"ExpansionTemplates are registered: this entry point does not expand generator objects -- review them through gk_review_batch, or "
-                      "aggregate the batch with gk_audit_add_batch, which do"};
     auto c = e->eng->compiled();
     ProgramLease lease(e, *c);
-    upload_blob(e, c, buf, offsets, n, source, flags & ~(uint32_t)GK_F_KEEP_SOURCE, &b, &stats);   // (the batch lives for this call only)
-    std::unique_ptr<gk_batch, std::function<void(gk_batch*)>> hold(b, [&](gk_batch* x) {
-      e->be->release(x->dev);
-      delete x;
-    });
-    eval_batch(e, b, ep, flags, out);
+    auto b = upload_blob(e, c, buf, offsets, n, source, flags & ~(uint32_t)GK_F_KEEP_SOURCE, &stats);   // (the batch lives for this call only)
+    eval_batch(e, b.get(), ep, flags, out);
     out->flatten_ms = stats.flatten_ms;
     out->h2d_ms = stats.h2d_ms;
     out->h2d_bytes = stats.h2d_bytes;
@@ -823,10 +850,7 @@ int gk_review_blob(gk_engine_t* e, const char* buf, const uint64_t* offsets, siz
 uint32_t gk_batch_size(gk_batch_t* b) { return b ? b->n : 0; }
 uint64_t gk_batch_alg_bytes(gk_batch_t* b) { return b ? b->alg_bytes : 0; }
 void gk_batch_free(gk_engine_t* e, gk_batch_t* b) {
-  if (!e || !b) return;
-  guard(nullptr, [&]() { e->be->release(b->dev); });
-  guard(nullptr, [&]() { e->be->release_source(b->source); });
-  delete b;
+  if (e) delete b;
 }
 
 int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err) {
@@ -835,10 +859,7 @@ int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err
   bool rebuilt = false;
   const int rc = guard(err, [&]() {
     auto c = e->eng->compiled();
-    const std::vector<std::string> excluded = excluded_of(e, b->flags);
-    uint64_t dv = 0;
-    if (c->uses_data) e->eng->data_doc(&dv);
-    if (c->version == b->compiled->version && excluded == b->excluded && (!c->uses_data || dv == b->data_version)) {
+    if (excluded_of(e, b->flags) == b->excluded && !stale_reason(e, *c, *b)) {
       if (stats) {
         stats->alg_bytes = b->alg_bytes;
         stats->n_objects = b->n;
@@ -847,18 +868,16 @@ int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err
       return;
     }
     ProgramLease lease(e, *c);
-    gk_batch* nb = nullptr;
-    if (!b->blob) upload_batch(e, c, b->objs.data(), b->objs.size(), b->flags, &nb, stats);
-    else if (b->source && device_ingest(*c, b->n)) refresh_from_source(e, c, b, &nb, stats);
-    else upload_blob(e, c, b->blob, b->blob_off, b->n, b->blob_source, b->flags, &nb, stats);
+    std::unique_ptr<gk_batch> nb;
+    if (!b->blob) nb = upload_batch(e, c, b->objs.data(), b->objs.size(), b->flags, stats);
+    else if (b->source && device_ingest(*c, b->n)) nb = refresh_from_source(e, c, *b, stats);
+    else nb = upload_blob(e, c, b->blob, b->blob_off, b->n, b->blob_source, b->flags, stats);
     // the new columns replace the old ones; a kept source stays with the batch (a batch that had none may have gained one)
     if (!nb->source) {
-      std::swap(nb->source, b->source);
-      std::swap(nb->source_errors, b->source_errors);
+      nb->source = std::move(b->source);
+      nb->source_errors = std::move(b->source_errors);
     }
-    std::swap(*b, *nb);
-    e->be->release(nb->dev);
-    delete nb;
+    std::swap(*b, *nb);   // (the old columns are released with nb)
     rebuilt = true;
   });
   return rc == GK_OK && rebuilt ? 1 : rc;
@@ -897,19 +916,14 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
   return guard(err, [&]() {
     gk_engine* e = a->e;
     auto c = e->eng->compiled();
-    if (c->version != b->compiled->version) throw RegoError{"batch was flattened against an older constraint set; upload it again"};
-    if (c->uses_data) {   // the columns of a referential snapshot hold values computed from data.inventory
-      uint64_t dv = 0;
-      e->eng->data_doc(&dv);
-      if (dv != b->data_version) throw RegoError{"data.inventory changed since the batch was flattened (referential constraints); upload it again"};
-    }
+    require_current(e, *c, *b);
     std::string ep = ep_c ? ep_c : "";
     std::vector<uint32_t> active;
     e->eng->active_mask(*c, ep, active);
     EvalOut ev, ev_amb;
     {
       ProgramLease lease(e, *c);
-      e->be->eval(b->dev, active, ev, true);
+      e->be->eval(b->dev.get(), active, ev, true);
     }
     std::vector<ObjIn> ins(b->n);
     for (size_t i = 0; i < ins.size(); ++i) ins[i] = b->obj_in(i);
@@ -917,18 +931,12 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
     // the pairs that have exactly one result and evaluate only what can still enter a constraint's list.
     BatchIdentity id;
     const bool lazy = !getenv("GK_AUDIT_EAGER") && (c->amb || std::any_of(c->single_result.begin(), c->single_result.end(), [](uint8_t x) { return x != 0; }));
-    if (lazy && !ordered) e->be->identity(b->dev, id);
+    if (lazy && !ordered) e->be->identity(b->dev.get(), id);
     const bool use_amb = lazy && (ordered || id.uniform_gvk) && c->amb && !getenv("GK_AUDIT_NO_AMB");
     if (use_amb) {
       ProgramLease lease(e, *c->amb);   // (the backend holds one netlist at a time: waits until no review uses the other)
-      void* fork = e->be->fork_batch(b->dev, *c->amb);
-      try {
-        e->be->eval(fork, active, ev_amb, true);
-      } catch (...) {
-        e->be->release(fork);
-        throw;
-      }
-      e->be->release(fork);
+      BackendHandle fork = device_batch(e, e->be->fork_batch(b->dev.get(), *c->amb));
+      e->be->eval(fork.get(), active, ev_amb, true);
     }
     // ---- expansion inside the audit loop (pkg/audit/manager.go:733-765): every reviewed object is expanded; its resultants are reviewed
     // as Generated resources with the parent's Namespace, their results -- "[Implied by <template>]", the template's action override --
@@ -936,46 +944,18 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
     // nothing at all, not even its own violations (the reference logs the error and `continue`s past the bookkeeping of the response).
     std::vector<std::string> obj_errs = b->host->obj_errors.empty() ? std::vector<std::string>(b->n) : b->host->obj_errors;
     obj_errs.resize(b->n);
-    struct Child {
-      uint32_t parent;
-      std::string json, tmpl, action;
-    };
-    std::vector<Child> children;
-    if (e->eng->has_expansion() && b->n) {
-      const size_t T = std::min<size_t>((size_t)std::max(1, e->eng->threads()), std::max<size_t>(1, b->n / 256));
-      std::vector<std::vector<Child>> part(T);
-      std::vector<std::vector<std::pair<uint32_t, std::string>>> perr(T);
-      auto work = [&](size_t t) {
-        std::vector<Resultant> res;
-        for (uint32_t i = (uint32_t)((size_t)b->n * t / T); i < (uint32_t)((size_t)b->n * (t + 1) / T); ++i) {
-          if (!obj_errs[i].empty()) continue;   // (the review of the object itself failed: the reference never gets to its expansion)
-          res.clear();
-          try {
-            e->eng->expand_object(ins[i], res);
-          } catch (std::exception& x) {
-            perr[t].emplace_back(i, std::string("unable to expand object: ") + x.what());
-            continue;
-          }
-          for (auto& r : res) part[t].push_back(Child{i, json_str(r.obj), r.template_name, r.action});
+    // (an object whose own review failed is not expanded: the reference never gets to its expansion)
+    const Expansion x = e->eng->has_expansion() ? expand_page(*e->eng, ins, obj_errs, e->eng->threads()) : Expansion();
+    const std::vector<Child>& children = x.children;
+    const uint32_t W = ev.words;
+    for (size_t i = 0; i < x.errors.size(); ++i)
+      if (!x.errors[i].empty()) {
+        obj_errs[i] = x.errors[i];
+        for (uint32_t w = 0; w < W; ++w) {
+          if (!ev.viol.empty()) ev.viol[i * W + w] = 0;
+          if (!ev.err.empty()) ev.err[i * W + w] = 0;
         }
-      };
-      if (T == 1) work(0);
-      else {
-        std::vector<std::thread> th;
-        for (size_t t = 0; t < T; ++t) th.emplace_back(work, t);
-        for (auto& x : th) x.join();
       }
-      const uint32_t W = ev.words;
-      for (auto& pe : perr)
-        for (auto& x : pe) {
-          obj_errs[x.first] = x.second;
-          for (uint32_t w = 0; w < W; ++w) {
-            if (!ev.viol.empty()) ev.viol[(size_t)x.first * W + w] = 0;
-            if (!ev.err.empty()) ev.err[(size_t)x.first * W + w] = 0;
-          }
-        }
-      for (auto& p : part) children.insert(children.end(), std::make_move_iterator(p.begin()), std::make_move_iterator(p.end()));
-    }
     // (after the expansion above: the rows of objects whose expansion failed are cleared, and they are no candidates either)
     std::vector<uint32_t> cand;
     if (lazy && ordered) {
@@ -985,35 +965,18 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
         } catch (JsonError&) {
         }
       };
-      e->be->audit_candidates(b->dev, ev.viol.data(), ev.words, (uint32_t)c->order.size(), (uint32_t)a->run.limit, gvk_of, cand, &a->select_ms);
+      e->be->audit_candidates(b->dev.get(), ev.viol.data(), ev.words, (uint32_t)c->order.size(), (uint32_t)a->run.limit, gvk_of, cand, &a->select_ms);
     }
     a->run.add_batch(*e->eng, *c, ins, ev.viol.data(), ev.err.empty() ? nullptr : ev.err.data(), ev.words, ev.errlist, ep,
                      lazy && !ordered ? &id : nullptr, use_amb ? ev_amb.viol.data() : nullptr, lazy && ordered ? cand.data() : nullptr);
     if (!children.empty()) {
-      std::vector<gk_obj> cobjs(children.size());
-      for (size_t k = 0; k < children.size(); ++k) {
-        gk_obj& o = cobjs[k];
-        memset(&o, 0, sizeof o);
-        o.json = children[k].json.data();
-        o.len = children[k].json.size();
-        const ObjIn& par = ins[children[k].parent];
-        o.ns_json = par.ns_json;                // the parent's Namespace object (manager.go:745-749), source Generated
-        o.ns_len = par.ns_len;
-        o.ns_name = par.ns_name;
-        o.source = GK_SOURCE_GENERATED;
-      }
-      gk_batch* cb = nullptr;
-      gk_result cstats, cres;
-      memset(&cstats, 0, sizeof cstats);
+      const std::vector<gk_obj> cobjs = resultant_objs(children, ins);
+      gk_result cres;
       memset(&cres, 0, sizeof cres);
       {
         ProgramLease lease(e, *c);
-        upload_batch(e, c, cobjs.data(), cobjs.size(), b->flags, &cb, &cstats);
-        std::unique_ptr<gk_batch, std::function<void(gk_batch*)>> hold(cb, [&](gk_batch* x) {
-          e->be->release(x->dev);
-          delete x;
-        });
-        eval_batch(e, cb, ep_c, GK_F_MATERIALIZE | GK_F_NO_COPY_BACK, &cres);
+        auto cb = upload_batch(e, c, cobjs.data(), cobjs.size(), b->flags, nullptr);
+        eval_batch(e, cb.get(), ep_c, GK_F_MATERIALIZE | GK_F_NO_COPY_BACK, &cres);
       }
       std::unique_ptr<ResultPriv> crp(static_cast<ResultPriv*>(cres.priv));
       cres.priv = nullptr;
