@@ -60,7 +60,7 @@ struct DevBatch {
   uint32_t words = 0;
   // tiling (depends on the batch's row distribution and on the program's slot table)
   uint32_t* d_tile_lo = nullptr;
-  uint32_t* d_tile_list = nullptr;   // [ntiles] tiles the specialised kernel hands to the interpreter (objects too big for its mask registers)
+  uint32_t* d_units = nullptr;       // [2 * n] object ranges the specialised kernel hands to the interpreter (GkKParams::units): never more than objects
   // the netlist with every slot id replaced by the slot's word offset in this batch's shared-memory slot area
   GkOp* d_ops = nullptr;
   uint32_t* d_pool = nullptr;
@@ -490,7 +490,7 @@ class CudaBackend : public Backend {
     push_small(db->d_pool, pool_r.data(), pool_r.size() * 4);
     push_small(db->d_outs, outs_r.data(), outs_r.size() * sizeof(GkOutEnt));
     db->words = std::max<uint32_t>(1, (uint32_t)((c.cons_match.size() + 31) / 32));
-    dmalloc(&db->d_tile_list, (size_t)(db->ntiles + 1) * 4);
+    dmalloc(&db->d_units, (size_t)db->n * 2 * 4);
     dmalloc(&db->viol, (size_t)std::max(db->n, 1u) * db->words * 4);
     dmalloc(&db->err, (size_t)std::max(db->n, 1u) * db->words * 4);
     CK(cudaStreamSynchronize(stream_));
@@ -541,7 +541,7 @@ class CudaBackend : public Backend {
     dfree(db->err);
     if (!db->fork) dfree(db->d_tile_lo);
     if (!db->fork) dfree(db->gvk);
-    dfree(db->d_tile_list);
+    dfree(db->d_units);
     dfree(db->d_ops);
     dfree(db->d_pool);
     dfree(db->d_outs);
@@ -583,8 +583,8 @@ class CudaBackend : public Backend {
       p.peer_tot[q] = nullptr;
     }
     p.timing = nullptr;
-    p.tile_list = db->d_tile_list;
-    p.tile_count = reinterpret_cast<uint32_t*>(d_scalars_) + 8;   // zeroed with the error counter before every launch
+    p.units = db->d_units;
+    p.unit_count = reinterpret_cast<uint32_t*>(d_scalars_) + 8;   // zeroed with the error counter before every launch
     p.list_mode = 0;
     p.pad_ = 0;
     spec_next_ = spec_ready(db->n);   // (an NVRTC run the first time: here, outside the timed region)
@@ -649,8 +649,8 @@ class CudaBackend : public Backend {
     uint32_t grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * per_sm)));
     last_kernel_ = "gk_eval_kernel";
     if (spec_next_) {
-      // the kernel generated for this constraint set does the tiles whose objects fit its mask registers (all of them, normally);
-      // the interpreter behind it takes the tiles it listed and, in the fused exchange, publishes the totals of both
+      // the kernel generated for this constraint set does the objects that fit its mask registers (all of them, normally); the
+      // interpreter behind it takes the object ranges it listed and, in the fused exchange, publishes the totals of both
       SpecEntry& se = *spec_cur_;
       uint32_t* xs = d_spec_x_;
       void* args[] = {&p, &xs};
@@ -667,10 +667,26 @@ class CudaBackend : public Backend {
       ++launches_;
       p.list_mode = 1;
       last_kernel_ = "gk_spec_kernel";
+      // how many units there are is known only on the device: the persistent grid, each CTA striding over the list
+      grid = std::max(1u, std::min<uint32_t>(p.batch.n, (uint32_t)(sms_ * per_sm)));
     }
     gk_eval_kernel<<<grid, kThreads, smem, st>>>(p);
     CK(cudaGetLastError());
     ++launches_;
+    if (p.list_mode && getenv("GK_TRACE_LAUNCH")) {   // (a read-back, so only when tracing)
+      uint32_t nu = 0;
+      CK(cudaMemcpyAsync(&nu, p.unit_count, 4, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      std::vector<uint32_t> u((size_t)nu * 2);
+      if (nu) CK(cudaMemcpy(u.data(), p.units, u.size() * 4, cudaMemcpyDeviceToHost));
+      uint64_t objs = 0, whole = 0;
+      for (uint32_t i = 0; i < nu; ++i) {
+        objs += u[2 * i + 1];
+        whole += u[2 * i + 1] > 1u;
+      }
+      fprintf(stderr, "[spec] handed to the interpreter: %u units (%llu of more than one object), %llu objects, on %u CTAs\n", nu, (unsigned long long)whole,
+              (unsigned long long)objs, grid);
+    }
   }
 
   // ---- the specialised kernel: source per constraint-set version (spec_codegen.cpp), compiled by NVRTC when first needed

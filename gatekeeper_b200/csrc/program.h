@@ -236,11 +236,20 @@ typedef struct {
   uint32_t tot_stride;
   uint32_t* done_ctr;
   unsigned long long* timing; // GK_PHASE_TIMING builds: [kMaxPhases + 2][2] = (CTA cycles between barriers, summed warp busy cycles)
-  // Tile list.  gk_spec_kernel keeps one mask word per netlist node and object, so an object may have at most 32 rows in a
-  // scope: a tile holding a bigger object is appended to tile_list (tile_count = its length) and left alone; gk_eval_kernel,
-  // launched behind it with list_mode = 1, evaluates exactly those tiles (and does the fused exchange's totals publication).
-  uint32_t* tile_list;
-  uint32_t* tile_count;
+  // Hand-over list.  gk_spec_kernel keeps one mask word per netlist node and object, so an object may have at most 32 rows in a
+  // scope.  A tile with up to GK_HANDOVER_MAX such wide objects appends each of them as a unit (object, 1) and counts the rest
+  // itself; a tile with more appends itself whole, (first object, objects), and counts nothing.  gk_eval_kernel, launched behind
+  // it with list_mode = 1, evaluates exactly those units (and does the fused exchange's totals publication).
+  uint32_t* units;            // [2 * unit capacity]: (first object, objects) pairs, each inside one tile
+  uint32_t* unit_count;
   uint32_t list_mode;
   uint32_t pad_;
 } GkKParams;
+// More wide objects than this in one tile hand the whole tile over.  A one-object unit pays the interpreter's per-phase barriers and
+// latencies for 1/512 of a tile's work.  Measured on an H100 over 1 M config-2 Pods with a wide object every 512 / 256 / 128 / 100
+// objects (1, 2, 4, ~5 per tile), one by one against whole tiles: 0.58 / 0.89 / 1.43 / 1.72 ms against 1.35 / 1.43 / 1.48 / 1.47.
+// So up to 4 go one by one.  (Defined from outside only to measure another value: tools/spec_probe.py --handover; 0 is the
+// whole-tile hand-over alone.)
+#ifndef GK_HANDOVER_MAX
+#define GK_HANDOVER_MAX 4u
+#endif

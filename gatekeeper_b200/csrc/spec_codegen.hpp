@@ -7,8 +7,8 @@
 // else reads (exports) are stored in shared memory.  Phase 2, one thread per OBJECT: every remaining node a 32-bit mask register
 // (bit j = row j of THIS object in the node's scope), an export that only object-level EXISTS read one bit of the OR of the rows'
 // words, EXISTS a `!= 0`, the object-major bitmap words assembled in registers without a transpose.  NVRTC compiles that text for
-// sm_90a when the first large batch is evaluated (kernels.cu).  Objects with more than 32 rows in some scope do not fit the mask registers: their tiles
-// are handed to the interpreter (GkKParams::tile_list).
+// sm_90a when the first large batch is evaluated (kernels.cu).  Objects with more than 32 rows in some scope do not fit the mask registers: they are
+// handed to the interpreter one by one, or with their whole tile when a tile holds more than GK_HANDOVER_MAX (GkKParams::units).
 #pragma once
 #include <string>
 #include <vector>

@@ -387,15 +387,15 @@ __global__ void __launch_bounds__(kThreads, GK_MIN_CTAS) gk_eval_kernel(const KP
   uint32_t* pool = reinterpret_cast<uint32_t*>(smem + L.pool);
   uint8_t* cbytes = reinterpret_cast<uint8_t*>(smem + L.cbytes);
 
-  // list mode (behind gk_spec_kernel): only the tiles that kernel left alone, usually none -- then nothing is staged
-  const uint32_t ntiles = p.list_mode ? *p.tile_count : p.ntiles;
+  // list mode (behind gk_spec_kernel): only the object ranges that kernel handed over, usually none -- then nothing is staged
+  const uint32_t nunits = p.list_mode ? *p.unit_count : p.ntiles;
   for (uint32_t i = threadIdx.x; i < C; i += blockDim.x) {
     s_tot[i] = 0;
     s_err[i] = 0;
     s_act[i] = p.active[i];
   }
   for (uint32_t i = threadIdx.x; i <= NP; i += blockDim.x) s_poff[i] = p.prog.phase_off[i];
-  if (ntiles) {   // the program and schema tables, each its whole padded region
+  if (blockIdx.x < nunits) {   // the program and schema tables, each its whole padded region
     stage(outs, p.prog.outs, L.ops - L.outs);
     stage(ops, p.prog.ops, L.items - L.ops);
     stage(items, p.prog.items, L.match - L.items);
@@ -410,13 +410,29 @@ __global__ void __launch_bounds__(kThreads, GK_MIN_CTAS) gk_eval_kernel(const KP
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   const uint32_t FULL = 0xffffffffu;
 
-  for (uint32_t ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
-    const uint32_t t = p.list_mode ? p.tile_list[ti] : ti;
-    // ---- tile row ranges (precomputed on the host: rows of a tile are contiguous at every scope)
-    for (uint32_t s = threadIdx.x; s < NS; s += blockDim.x) {
-      const uint32_t a = p.tile_lo[(size_t)t * NS + s], b = p.tile_lo[(size_t)(t + 1) * NS + s];
-      s_lo[s] = a;
-      s_cnt[s] = b - a;
+  for (uint32_t ti = blockIdx.x; ti < nunits; ti += gridDim.x) {
+    // ---- the unit's row ranges (rows of consecutive objects are contiguous at every scope): a tile's from the precomputed table;
+    // a listed object range's through the CSR offsets, parents before children (any such range lies inside one tile, so the slot
+    // area sized for the largest tile holds it)
+    if (p.list_mode) {
+      if (threadIdx.x == 0) {
+        const uint32_t a = p.units[2 * ti];
+        uint32_t* s_hi = s_cnt;   // (the range ends first, turned into counts below)
+        s_lo[0] = a;
+        s_hi[0] = a + p.units[2 * ti + 1];
+        for (uint32_t s = 1; s < NS; ++s) {
+          const uint32_t par = (uint32_t)scopes[s].parent;
+          s_lo[s] = scopes[s].off[s_lo[par]];
+          s_hi[s] = scopes[s].off[s_hi[par]];
+        }
+        for (uint32_t s = 0; s < NS; ++s) s_cnt[s] -= s_lo[s];
+      }
+    } else {
+      for (uint32_t s = threadIdx.x; s < NS; s += blockDim.x) {
+        const uint32_t a = p.tile_lo[(size_t)ti * NS + s], b = p.tile_lo[(size_t)(ti + 1) * NS + s];
+        s_lo[s] = a;
+        s_cnt[s] = b - a;
+      }
     }
     __syncthreads();
     const uint32_t nobj = s_cnt[0], obj0 = s_lo[0];

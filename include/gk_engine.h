@@ -105,7 +105,8 @@ void gk_engine_destroy(gk_engine_t* e);
 const char* gk_backend_name(gk_engine_t* e);
 /* Which kernel decided the engine's last evaluation: "gk_spec_kernel" (CUDA C++ generated from the constraint set's netlist and
  * compiled by NVRTC for sm_90a the first time a batch of >= GK_SPEC_MIN_OBJECTS objects meets the set; GK_SPEC=0 turns it off)
- * or "gk_eval_kernel" (the netlist interpreter: small batches, and tiles holding an object with more than 32 rows in a scope).
+ * or "gk_eval_kernel" (the netlist interpreter: small batches, and objects with more than 32 rows in a scope -- with their whole
+ * tile when a tile holds many of them).
  * Replaces nothing in the reference: frameworks' rego driver compiles a template's Rego once per AddTemplate
  * (pkg/drivers/k8scel/driver.go:79-146 is the CEL analogue in this tree); this is the per-constraint-set analogue on the device. */
 const char* gk_last_kernel(gk_engine_t* e);
