@@ -12,9 +12,11 @@
 #include <new>
 #include <utility>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "engine.hpp"
+#include "fold_core.h"
 #include "program.h"
 
 namespace gk {
@@ -71,6 +73,7 @@ struct DevOutPtrs {          // caller-owned device buffers (e.g. torch tensors)
   uint64_t peer_viol[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   uint64_t peer_tot[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   uint32_t npeers = 0, tot_stride = 0;
+  uint32_t rank = 0;         // which of the peers this rank is (its own slot holds its unfolded rows: Backend::fold_into)
 };
 
 // What orders audit results besides the message: group / version / kind, namespace, name (pkg/audit/manager.go:161-202).  Read
@@ -104,6 +107,9 @@ class Backend {
   virtual void* ingest_keep(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status, void** keep);
   virtual void* reextract(void* source, const IngestReq& rq, IngestStats* st);
   virtual void release_source(void* source);
+  // The JSON of objects `idx` of a kept page source, back to back into `bytes`, object k at [off[k], off[k+1]) (an expanded batch's
+  // refresh, which does not read the caller's page).  The CUDA backend gathers them from the page's device copy.
+  virtual void source_bytes(void* source, const std::vector<uint32_t>& idx, std::string& bytes, std::vector<uint64_t>& off);
   virtual void identity(void* batch, BatchIdentity& out) = 0;
   // The audit's candidates of a reviewed batch for any mix of kinds (gk_audit_add_batch_ordered).  Objects are ordered by (group,
   // version, kind, namespace, name) as sv_less orders results (namespace and name as BatchIdentity holds them); for constraint c the
@@ -114,6 +120,28 @@ class Backend {
   using GvkOf = std::function<void(uint32_t object, std::string& group, std::string& version, std::string& kind)>;
   virtual void audit_candidates(void* batch, const uint32_t* viol, uint32_t words, uint32_t nconstraints, uint32_t limit, const GvkOf& gvk_of,
                                 std::vector<uint32_t>& cand, float* device_ms);
+  // ---- expanded batches (GK_F_EXPAND, gk_engine.h).  The defaults run on the host: for a backend whose batches are host memory and
+  // whose "device" output buffers are host memory too (the test-only host emulation).
+  // Generator selection: the objects of `batch` that may have resultants, ascending, into `sel`: those whose (group, version, kind)
+  // -- decoded by `gvk_of` -- `wanted` keeps.  `kinds`: how many distinct kinds were decoded.  The CUDA backend decodes one object per
+  // distinct apiVersion / kind hash of the batch, marks and compacts the objects on the device, and selects every object without a
+  // hash (skipped by the excluder, no object, the old object of a DELETE) as well; this default decodes every object.
+  using GvkWanted = std::function<bool(const std::string& group, const std::string& version, const std::string& kind)>;
+  virtual void select_generators(void* batch, const GvkOf& gvk_of, const GvkWanted& wanted, std::vector<uint32_t>& sel, uint32_t* kinds,
+                                 float* device_ms);
+  // The parents of resultant batch `res`, a CSR over the parents that have resultants: par[j] has resultants off[j] .. off[j+1]-1.
+  // The same vectors are passed to eval_expanded / fold_into; a backend that keeps its own copy (the CUDA backend: in device memory)
+  // takes it here.  The default keeps nothing.
+  virtual void set_parents(void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off) { (void)res, (void)par, (void)off; }
+  // gk_batch_eval of an expanded batch: `batch`, then its resultant batch `res`, then every resultant's rows ORed into its parent's;
+  // `out` receives the folded planes (when copy_back), the parents' matcher-error list, and totals / kernel time that include the
+  // resultants and the fold.  `own` (may be null): the parents' unfolded planes; `rout` (may be null): the resultants' evaluation.
+  virtual void eval_expanded(void* batch, void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off,
+                             const std::vector<uint32_t>& active, EvalOut& out, bool copy_back, EvalOut* own, EvalOut* rout);
+  // After eval_into(batch, active, dst): evaluates `res` into its own planes and folds them into every destination of `dst` (the
+  // unfolded rows are read from dst.viol, or from this rank's slot dst.peer_viol[dst.rank]; dst.err), on dst.stream, unsynchronised.
+  virtual void fold_into(void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off, const std::vector<uint32_t>& active,
+                         const DevOutPtrs& dst);
   // A second view of a resident batch for ANOTHER netlist over the same schema (Compiled::amb): shares the columns, owns its
   // own slot-resolved netlist and output planes.  Evaluate it with eval() while the backend holds `other`; release() it before
   // the batch it was forked from.
@@ -153,6 +181,106 @@ inline void* Backend::reextract(void* source, const IngestReq& rq, IngestStats* 
   return ingest(r, st, &status);
 }
 inline void Backend::release_source(void* source) { delete static_cast<HostPageCopy*>(source); }
+inline void Backend::source_bytes(void* source, const std::vector<uint32_t>& idx, std::string& bytes, std::vector<uint64_t>& off) {
+  auto* src = static_cast<HostPageCopy*>(source);
+  bytes.clear();
+  off.assign(1, 0);
+  for (uint32_t i : idx) {
+    if (!src || (size_t)i + 1 >= src->ooff.size()) throw BackendError{"kept source: object index out of range"};
+    bytes.append(reinterpret_cast<const char*>(src->blob.data()) + src->ooff[i], (size_t)(src->ooff[i + 1] - src->ooff[i]));
+    off.push_back(bytes.size());
+  }
+}
+
+// the fold of resultant planes `cviol` / `cerr` into parents by the CSR (par, off), on host arrays; the caller fills in the rest
+inline GkFoldArgs fold_args_host(const std::vector<uint32_t>& par, const std::vector<uint32_t>& off, const EvalOut& res, uint32_t words,
+                                 uint32_t nconstraints) {
+  if (off.size() != par.size() + 1) throw BackendError{"fold: the offsets must have one entry more than the parents"};
+  if (!off.empty() && (size_t)off.back() * words > res.viol.size()) throw BackendError{"fold: more resultants than the resultant batch holds"};
+  GkFoldArgs a{};
+  a.par = par.data();
+  a.off = off.data();
+  a.m = (uint32_t)par.size();
+  a.words = words;
+  a.nconstraints = nconstraints;
+  a.cviol = res.viol.data();
+  a.cerr = res.err.data();
+  return a;
+}
+
+// every parent of `a` in turn (the rule gk_fold_kernel runs one thread per parent), then the totals of the fused exchange
+// published to every peer
+inline void fold_host(const GkFoldArgs& a) {
+  for (uint32_t j = 0; j < a.m; ++j)
+    gk_fold_parent(a, j, [&](uint32_t c, uint32_t plane) {
+      if (c < a.nconstraints) ++(plane ? a.err_totals : a.totals)[c];
+    });
+  for (uint32_t q = 0; q < a.npeers; ++q)
+    for (uint32_t c = 0; c < a.nconstraints; ++c) {
+      a.peer_tot[q][c] = a.totals[c];
+      a.peer_tot[q][a.tot_stride + c] = a.err_totals[c];
+    }
+}
+
+inline void Backend::select_generators(void* batch, const GvkOf& gvk_of, const GvkWanted& wanted, std::vector<uint32_t>& sel, uint32_t* kinds,
+                                       float* device_ms) {
+  BatchIdentity id;
+  identity(batch, id);
+  std::unordered_map<std::string, bool> seen;
+  sel.clear();
+  for (uint32_t o = 0; o < (uint32_t)id.flags.size(); ++o) {
+    std::string g, v, k;
+    gvk_of(o, g, v, k);
+    auto it = seen.find(g + '\0' + v + '\0' + k);
+    if (it == seen.end()) it = seen.emplace(g + '\0' + v + '\0' + k, wanted(g, v, k)).first;
+    if (it->second) sel.push_back(o);
+  }
+  if (kinds) *kinds = (uint32_t)seen.size();
+  if (device_ms) *device_ms = 0.f;
+}
+
+inline void Backend::eval_expanded(void* batch, void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off,
+                                   const std::vector<uint32_t>& active, EvalOut& out, bool copy_back, EvalOut* own, EvalOut* rout) {
+  (void)copy_back;   // (the planes are on the host anyway)
+  eval(batch, active, out, true);
+  EvalOut tmp;
+  EvalOut& r = rout ? *rout : tmp;
+  eval(res, active, r, true);
+  if (own) {
+    own->viol = out.viol;
+    own->err = out.err;
+  }
+  const uint32_t C = out.nconstraints;
+  GkFoldArgs a = fold_args_host(par, off, r, out.words, C);
+  a.sviol = a.dviol = out.viol.data();
+  a.serr = a.derr = out.err.data();
+  std::vector<unsigned long long> t(2 * (size_t)C + 1, 0);
+  a.totals = t.data();
+  a.err_totals = t.data() + C;
+  fold_host(a);
+  for (uint32_t c = 0; c < C; ++c) out.totals[c] += t[c], out.err_totals[c] += t[C + c];
+  out.kernel_ms += r.kernel_ms;
+}
+
+inline void Backend::fold_into(void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off, const std::vector<uint32_t>& active,
+                               const DevOutPtrs& dst) {
+  if (dst.npeers > GK_MAX_PEERS || (dst.npeers && dst.rank >= dst.npeers)) throw BackendError{"fold: bad peer addressing"};
+  EvalOut r;
+  eval(res, active, r, true);
+  GkFoldArgs a = fold_args_host(par, off, r, r.words, r.nconstraints);
+  a.sviol = dst.npeers ? reinterpret_cast<const uint32_t*>(dst.peer_viol[dst.rank]) : static_cast<const uint32_t*>(dst.viol);
+  a.serr = a.derr = static_cast<uint32_t*>(dst.err);
+  a.dviol = dst.npeers ? nullptr : static_cast<uint32_t*>(dst.viol);
+  a.npeers = dst.npeers;
+  a.tot_stride = dst.tot_stride;
+  for (uint32_t q = 0; q < dst.npeers; ++q) {
+    a.peer_viol[q] = reinterpret_cast<uint32_t*>(dst.peer_viol[q]);
+    a.peer_tot[q] = reinterpret_cast<unsigned long long*>(dst.peer_tot[q]);
+  }
+  a.totals = static_cast<unsigned long long*>(dst.totals);
+  a.err_totals = static_cast<unsigned long long*>(dst.err_totals);
+  fold_host(a);
+}
 
 // ---- arena packing shared by both backends: every array of a HostBatch laid out contiguously
 struct PackedBatch {

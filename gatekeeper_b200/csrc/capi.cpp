@@ -128,6 +128,8 @@ struct BackendRelease {
 };
 using BackendHandle = std::unique_ptr<void, BackendRelease>;
 
+struct Expanded;   // an expanded batch's resultants (GK_F_EXPAND), below
+
 BackendHandle device_batch(gk_engine* e, void* dev) { return BackendHandle(dev, BackendRelease{e->be.get(), &Backend::release}); }
 BackendHandle kept_source(gk_engine* e, void* source) { return BackendHandle(source, BackendRelease{e->be.get(), &Backend::release_source}); }
 }  // namespace
@@ -151,10 +153,34 @@ struct gk_batch {
   // review-level errors of its objects (they depend on the page alone)
   BackendHandle source;
   std::vector<std::string> source_errors;
+  std::shared_ptr<Expanded> ex;        // GK_F_EXPAND: the page's resultants (null: a batch uploaded without the flag)
   ObjIn obj_in(size_t i) const;
 };
 
 namespace {
+
+// ---- expansion (pkg/audit/manager.go:733-765, pkg/webhook/policy.go:610-646), the step gk_review_batch, the expanded batches and the
+// audit share: the resultants of generator objects are reviewed as generated resources, and their results folded back onto their parents
+struct Child {
+  uint32_t parent;
+  std::string json, tmpl, action;
+};
+
+struct Expansion {
+  std::vector<Child> children;       // in object order
+  std::vector<std::string> errors;   // per object: "" or why its expansion failed
+};
+
+// An expanded batch's resultants: a resident batch of their own, in parent order, and what folds them onto their parents
+struct Expanded {
+  uint64_t version = 0;              // Engine::expansion_version the page was expanded at
+  Expansion x;                       // children[k].parent: an object of the parent batch; errors: [parents] or empty
+  std::string blob;                  // blob parents: the resultants' JSON as one page ...
+  std::vector<uint64_t> off;         // ... and its offsets
+  std::vector<gk_obj> objs;          // object parents: the resultants as review objects (their JSON in x.children)
+  std::unique_ptr<gk_batch> res;     // null: the page has no resultants
+  std::vector<uint32_t> par, off_par;   // its parents, a CSR over the parents that have resultants (Backend::set_parents)
+};
 
 struct ResultPriv {
   std::shared_ptr<const Compiled> compiled;   // the snapshot the result was computed with (constraint indices refer to it)
@@ -262,7 +288,90 @@ void fill_result(gk_result* out, ResultPriv* rp, bool have_bits) {
   out->priv = rp;
 }
 
-// evaluate a resident batch; optionally render messages for flagged pairs
+// The results of every flagged pair of batch `b`'s rows in `viol` / `err` (its evaluation's matcher-error list `errlist`): matcher errors
+// first (autoreject results), then rendered violations, both in (object, constraint) order
+std::vector<Violation> render(gk_engine* e, const Compiled& c, const gk_batch& b, const BitPlane& viol, const BitPlane& err, const std::vector<uint32_t>& errlist,
+                              uint32_t W, uint32_t C, const std::string& ep) {
+  std::vector<Violation> vio;
+  std::unordered_map<uint64_t, uint32_t> err_code;
+  for (size_t i = 0; i + 2 < errlist.size(); i += 3) err_code[((uint64_t)errlist[i] << 32) | errlist[i + 1]] = errlist[i + 2];
+  // one DOM parse per object, all of its flagged constraints rendered from it; objects are spread over the host threads
+  const uint32_t n = b.n;
+  const size_t T = std::min<size_t>((size_t)std::max(1, e->eng->threads()), std::max<size_t>(1, n / 16));
+  std::vector<std::vector<Violation>> part(T);
+  std::vector<std::string> errs(T);
+  auto work = [&](size_t t) {
+    std::vector<Engine::Flagged> flagged;
+    Engine::MaterializeCtx mctx;
+    try {
+      for (uint32_t o = (uint32_t)(n * t / T); o < (uint32_t)(n * (t + 1) / T); ++o) {
+        flagged.clear();
+        for (uint32_t w = 0; w < W; ++w) {
+          const uint32_t vb = viol[(size_t)o * W + w], eb = err[(size_t)o * W + w];
+          uint32_t any = vb | eb;
+          while (any) {
+            const uint32_t k = (uint32_t)__builtin_ctz(any);
+            any &= any - 1;
+            const uint32_t cix = w * 32 + k;
+            if (cix >= C) continue;
+            const bool is_err = eb >> k & 1u;
+            uint32_t code = 0;
+            if (is_err) {
+              auto it = err_code.find(((uint64_t)o << 32) | c.cons_match[cix]);   // error list is keyed by match block
+              if (it != err_code.end()) code = it->second;
+            }
+            flagged.push_back({cix, is_err, code});
+          }
+        }
+        if (!flagged.empty()) e->eng->materialize_object(c, b.obj_in(o), o, flagged, ep, part[t], nullptr, &mctx);
+      }
+    } catch (RegoError& x) {
+      errs[t] = x.msg;
+    } catch (std::exception& x) {
+      errs[t] = x.what();
+    }
+  };
+  if (T == 1) work(0);
+  else {
+    std::vector<std::thread> th;
+    for (size_t t = 0; t < T; ++t) th.emplace_back(work, t);
+    for (auto& x : th) x.join();
+  }
+  for (auto& x : errs)
+    if (!x.empty()) throw RegoError{x};
+  for (auto& v : part) vio.insert(vio.end(), std::make_move_iterator(v.begin()), std::make_move_iterator(v.end()));
+  return vio;
+}
+
+// The resultants' results and review-level errors reported on their parents (aggregate.go:19-63): `vio` holds the results of the
+// parents 0 .. n-1 and those of resultant k as object n + k, `obj_errors` the review-level errors of the same rows (empty: none).
+// Results are re-indexed with "[Implied by <template>]" and the template's enforcement-action override, a resultant's review-level
+// error is reported on its parent, and so is a failed expansion (`expand_errors`: per parent, or empty).
+void fold_results(std::vector<Violation>& vio, std::vector<std::string>& obj_errors, size_t n, const std::vector<Child>& children,
+                  const std::vector<std::string>& expand_errors) {
+  for (auto& v : vio)
+    if (v.object >= n) {
+      const Child& ch = children[v.object - n];
+      v.object = ch.parent;
+      v.msg = ExpansionSystem::implied_by(ch.tmpl, v.msg);
+      if (!ch.action.empty()) v.action = ch.action;   // OverrideEnforcementAction (aggregate.go:47-58) sets EnforcementAction only: the scoped list stays
+    }
+  std::stable_sort(vio.begin(), vio.end(), [](const Violation& a, const Violation& b2) { return a.object < b2.object; });
+  const bool any_expand_err = std::any_of(expand_errors.begin(), expand_errors.end(), [](const std::string& m) { return !m.empty(); });
+  if (obj_errors.empty() && any_expand_err) obj_errors.assign(n + children.size(), std::string());
+  if (!obj_errors.empty()) {
+    for (size_t k = 0; k < children.size(); ++k)
+      if (!obj_errors[n + k].empty() && obj_errors[children[k].parent].empty())
+        obj_errors[children[k].parent] = ExpansionSystem::implied_by(children[k].tmpl, obj_errors[n + k]);
+    obj_errors.resize(n);
+    for (size_t i = 0; i < n && i < expand_errors.size(); ++i)
+      if (!expand_errors[i].empty() && obj_errors[i].empty()) obj_errors[i] = expand_errors[i];
+  }
+}
+
+// evaluate a resident batch; optionally render messages for flagged pairs.  An expanded batch: the parents, then the resultants, then
+// the fold of the resultants' rows into the parents' rows on the device; the results are rendered from the unfolded rows and folded
+// as gk_review_batch folds them.
 void eval_batch(gk_engine* e, gk_batch* b, const char* ep_c, uint32_t flags, gk_result* out) {
   std::string ep = ep_c ? ep_c : "";
   const Compiled& c = *b->compiled;
@@ -271,69 +380,42 @@ void eval_batch(gk_engine* e, gk_batch* b, const char* ep_c, uint32_t flags, gk_
   for (auto* k : c.order) rp->keys.push_back(k->kind + "/" + k->name);
   std::vector<uint32_t> active;
   e->eng->active_mask(c, ep, active);
-  bool copy_back = !(flags & GK_F_NO_COPY_BACK) || (flags & GK_F_MATERIALIZE);
+  const bool materialize = (flags & GK_F_MATERIALIZE) != 0;
+  bool copy_back = !(flags & GK_F_NO_COPY_BACK) || materialize;
+  const gk_batch* res = b->ex ? b->ex->res.get() : nullptr;
   double t0 = now_ms();
-  e->be->eval(b->dev.get(), active, rp->ev, copy_back);
+  EvalOut own, rev;   // the parents' unfolded rows and the resultants' own rows (materialize)
+  if (res) e->be->eval_expanded(b->dev.get(), res->dev.get(), b->ex->par, b->ex->off_par, active, rp->ev, copy_back, materialize ? &own : nullptr,
+                                materialize ? &rev : nullptr);
+  else e->be->eval(b->dev.get(), active, rp->ev, copy_back);
   double t1 = now_ms();
   rp->obj_errors = b->host->obj_errors;
   out->d2h_bytes = copy_back ? (uint64_t)rp->ev.viol.size() * 8 : 0;
   out->d2h_ms = (t1 - t0) - rp->ev.kernel_ms;
   if (out->d2h_ms < 0) out->d2h_ms = 0;
-  out->alg_bytes = b->alg_bytes + (uint64_t)b->n * rp->ev.words * 8;
+  out->alg_bytes = b->alg_bytes + (uint64_t)(b->n + (res ? res->n : 0)) * rp->ev.words * 8;
   out->materialize_ms = 0;
-  if (flags & GK_F_MATERIALIZE) {
+  if (materialize) {
     double m0 = now_ms();
     const uint32_t W = rp->ev.words, C = rp->ev.nconstraints;
-    // matcher errors first (autoreject results), then rendered violations, both in (object, constraint) order
-    std::unordered_map<uint64_t, uint32_t> err_code;
-    for (size_t i = 0; i + 2 < rp->ev.errlist.size(); i += 3)
-      err_code[((uint64_t)rp->ev.errlist[i] << 32) | rp->ev.errlist[i + 1]] = rp->ev.errlist[i + 2];
-    // one DOM parse per object, all of its flagged constraints rendered from it; objects are spread over the host threads
-    const uint32_t n = b->n;
-    const size_t T = std::min<size_t>((size_t)std::max(1, e->eng->threads()), std::max<size_t>(1, n / 16));
-    std::vector<std::vector<Violation>> part(T);
-    std::vector<std::string> errs(T);
-    auto work = [&](size_t t) {
-      std::vector<Engine::Flagged> flagged;
-      Engine::MaterializeCtx mctx;
-      try {
-        for (uint32_t o = (uint32_t)(n * t / T); o < (uint32_t)(n * (t + 1) / T); ++o) {
-          flagged.clear();
-          for (uint32_t w = 0; w < W; ++w) {
-            const uint32_t vb = rp->ev.viol[(size_t)o * W + w], eb = rp->ev.err[(size_t)o * W + w];
-            uint32_t any = vb | eb;
-            while (any) {
-              const uint32_t k = (uint32_t)__builtin_ctz(any);
-              any &= any - 1;
-              const uint32_t cix = w * 32 + k;
-              if (cix >= C) continue;
-              const bool is_err = eb >> k & 1u;
-              uint32_t code = 0;
-              if (is_err) {
-                auto it = err_code.find(((uint64_t)o << 32) | c.cons_match[cix]);   // error list is keyed by match block
-                if (it != err_code.end()) code = it->second;
-              }
-              flagged.push_back({cix, is_err, code});
-            }
-          }
-          if (!flagged.empty()) e->eng->materialize_object(c, b->obj_in(o), o, flagged, ep, part[t], nullptr, &mctx);
-        }
-      } catch (RegoError& x) {
-        errs[t] = x.msg;
-      } catch (std::exception& x) {
-        errs[t] = x.what();
-      }
-    };
-    if (T == 1) work(0);
-    else {
-      std::vector<std::thread> th;
-      for (size_t t = 0; t < T; ++t) th.emplace_back(work, t);
-      for (auto& x : th) x.join();
+    rp->vio = render(e, c, *b, res ? own.viol : rp->ev.viol, res ? own.err : rp->ev.err, rp->ev.errlist, W, C, ep);
+    if (res) {
+      std::vector<Violation> rv = render(e, c, *res, rev.viol, rev.err, rev.errlist, W, C, ep);
+      for (auto& v : rv) v.object += b->n;
+      rp->vio.insert(rp->vio.end(), std::make_move_iterator(rv.begin()), std::make_move_iterator(rv.end()));
     }
-    for (auto& x : errs)
-      if (!x.empty()) throw RegoError{x};
-    for (auto& v : part) rp->vio.insert(rp->vio.end(), std::make_move_iterator(v.begin()), std::make_move_iterator(v.end()));
     out->materialize_ms = now_ms() - m0;
+  }
+  if (b->ex) {
+    const Expanded& x = *b->ex;
+    if (res && !res->host->obj_errors.empty()) {
+      rp->obj_errors.resize(b->n);
+      rp->obj_errors.insert(rp->obj_errors.end(), res->host->obj_errors.begin(), res->host->obj_errors.end());
+      rp->obj_errors.resize((size_t)b->n + x.x.children.size());
+    } else if (!rp->obj_errors.empty()) {
+      rp->obj_errors.resize((size_t)b->n + x.x.children.size());
+    }
+    fold_results(rp->vio, rp->obj_errors, b->n, x.x.children, x.x.errors);
   }
   bool give_bits = !(flags & GK_F_NO_COPY_BACK);
   fill_result(out, rp.release(), give_bits);
@@ -491,28 +573,7 @@ void require_current(gk_engine* e, const Compiled& c, const gk_batch& b) {
   if (const char* why = stale_reason(e, c, b)) throw RegoError{why};
 }
 
-// gk_batch_eval_device and gk_batch_eval_device_peers: the kernel's outputs go to the caller's device buffers `d`
-void eval_device(gk_engine* e, const gk_batch& b, const char* ep, const DevOutPtrs& d) {
-  refuse_while_expanding(e);
-  auto c = e->eng->compiled();
-  require_current(e, *c, b);
-  ProgramLease lease(e, *c);
-  std::vector<uint32_t> active;
-  e->eng->active_mask(*c, ep ? ep : "", active);
-  e->be->eval_into(b.dev.get(), active, d);
-}
 
-// ---- expansion (pkg/audit/manager.go:733-765, pkg/webhook/policy.go:610-646), the step gk_review_batch and the audit share: the
-// resultants of generator objects are reviewed as generated resources, and their results folded back onto their parents
-struct Child {
-  uint32_t parent;
-  std::string json, tmpl, action;
-};
-
-struct Expansion {
-  std::vector<Child> children;       // in object order
-  std::vector<std::string> errors;   // per object: "" or why its expansion failed
-};
 
 // Expands every object of `ins` but those with a non-empty skip[i] (`skip` may be empty); a large page is spread over the host threads.
 Expansion expand_page(Engine& eng, const std::vector<ObjIn>& ins, const std::vector<std::string>& skip, int threads) {
@@ -569,6 +630,117 @@ std::vector<gk_obj> resultant_objs(const std::vector<Child>& children, const std
   return v;
 }
 
+// the (group, version, kind) of a review's generator -- the old object of a DELETE, as Engine::expand_object expands it; empty when
+// it has none or it is not a JSON object
+void generator_gvk(const ObjIn& in, std::string& g, std::string& v, std::string& k) {
+  const bool del = in.operation && std::string(in.operation) == "DELETE";
+  const char* gj = del ? in.old_json : in.json;
+  if (!gj) return;
+  try {
+    VP o = json_parse(gj, del ? in.old_len : in.len);
+    if (o && o->t == VT::Obj) split_gv(o, g, v, k);
+  } catch (JsonError&) {
+  }
+}
+
+// GK_F_EXPAND, after the upload of batch `b` against snapshot `c`: the generators are selected on the device, expanded on the host, and
+// their resultants uploaded as the batch's resultant batch.  `version`: the expansion version read before the parents were flattened.
+// `from_source`: the parents' JSON comes from the batch's kept source (a refresh does not read the caller's page).
+void expand_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, gk_batch& b, uint64_t version, bool from_source) {
+  auto ex = std::make_shared<Expanded>();
+  ex->version = version;
+  b.ex = ex;
+  if (!b.n || !e->eng->has_expansion()) return;
+  std::string kept;   // from_source: the gathered JSON of the objects being read
+  std::vector<uint64_t> kept_off;
+  auto fetch = [&](const std::vector<uint32_t>& idx) {
+    std::vector<ObjIn> ins(idx.size());
+    if (from_source) {
+      e->be->source_bytes(b.source.get(), idx, kept, kept_off);
+      for (size_t i = 0; i < idx.size(); ++i) {
+        ins[i].json = kept.data() + kept_off[i];
+        ins[i].len = (size_t)(kept_off[i + 1] - kept_off[i]);
+        ins[i].source = b.blob_source;
+      }
+    } else {
+      for (size_t i = 0; i < idx.size(); ++i) ins[i] = b.obj_in(idx[i]);
+    }
+    return ins;
+  };
+  const double t0 = now_ms();
+  std::vector<uint32_t> sel;
+  uint32_t kinds = 0;
+  float sel_ms = 0.f;
+  e->be->select_generators(
+      b.dev.get(), [&](uint32_t o, std::string& g, std::string& v, std::string& k) { generator_gvk(fetch({o})[0], g, v, k); },
+      [e](const std::string& g, const std::string& v, const std::string& k) { return e->eng->expansion_selects(g, v, k); }, sel, &kinds, &sel_ms);
+  const double t1 = now_ms();
+  const std::vector<ObjIn> ins = fetch(sel);
+  Expansion x = expand_page(*e->eng, ins, {}, e->eng->threads());
+  const double t2 = now_ms();
+  std::vector<gk_obj> robjs = resultant_objs(x.children, ins);
+  for (auto& ch : x.children) ch.parent = sel[ch.parent];
+  if (std::any_of(x.errors.begin(), x.errors.end(), [](const std::string& m) { return !m.empty(); })) {
+    ex->x.errors.assign(b.n, std::string());
+    for (size_t i = 0; i < sel.size(); ++i) ex->x.errors[sel[i]] = std::move(x.errors[i]);
+  }
+  const size_t m = x.children.size();
+  const uint32_t rflags = b.flags & ~(uint32_t)(GK_F_KEEP_SOURCE | GK_F_EXPAND);
+  if (m) {
+    if (b.blob) {   // blob parents (no Namespace objects): the resultants as one page, for the device ingest
+      ex->off.assign(1, 0);
+      for (auto& ch : x.children) {
+        ex->blob += ch.json;
+        ex->off.push_back(ex->blob.size());
+        std::string().swap(ch.json);
+      }
+      robjs.clear();
+      ex->res = upload_blob(e, c, ex->blob.data(), ex->off.data(), m, GK_SOURCE_GENERATED, rflags, nullptr);
+    } else {
+      ex->objs = std::move(robjs);
+      ex->res = upload_batch(e, c, ex->objs.data(), m, rflags, nullptr);
+    }
+    std::vector<uint32_t>& par = ex->par;
+    std::vector<uint32_t>& off = ex->off_par;
+    off.assign(1, 0);
+    for (size_t k = 0; k < m; ++k) {
+      if (par.empty() || par.back() != x.children[k].parent) {
+        if (!par.empty()) off.push_back((uint32_t)k);
+        par.push_back(x.children[k].parent);
+      }
+    }
+    off.push_back((uint32_t)m);
+    e->be->set_parents(ex->res->dev.get(), par, off);
+    b.alg_bytes += ex->res->alg_bytes;
+  }
+  ex->x.children = std::move(x.children);
+  if (getenv("GK_TRACE_LAUNCH"))
+    fprintf(stderr, "[expand] %u objects, %u distinct kinds, %zu selected, %zu resultants; selection %.3f ms on the device (%.3f ms wall), expansion %.3f ms, resultant upload %.3f ms\n",
+            b.n, kinds, sel.size(), m, sel_ms, t1 - t0, t2 - t1, now_ms() - t2);
+}
+
+// the eval calls' check of an expanded batch (and their refusal of any other batch while templates are registered)
+bool expansion_stale(gk_engine* e, const gk_batch& b) { return b.ex && b.ex->version != e->eng->expansion_version(); }
+void require_expanded_or_none(gk_engine* e, const gk_batch& b) {
+  if (!b.ex) refuse_while_expanding(e);
+  else if (expansion_stale(e, b)) throw RegoError{"ExpansionTemplates changed since the batch was expanded; refresh it with gk_batch_refresh or upload it again"};
+}
+
+}  // namespace
+
+namespace {
+// gk_batch_eval_device and gk_batch_eval_device_peers: the kernel's outputs go to the caller's device buffers `d` (an expanded batch:
+// then its resultants' evaluation and the fold, on the same stream)
+void eval_device(gk_engine* e, const gk_batch& b, const char* ep, const DevOutPtrs& d) {
+  require_expanded_or_none(e, b);
+  auto c = e->eng->compiled();
+  require_current(e, *c, b);
+  ProgramLease lease(e, *c);
+  std::vector<uint32_t> active;
+  e->eng->active_mask(*c, ep ? ep : "", active);
+  e->be->eval_into(b.dev.get(), active, d);
+  if (b.ex && b.ex->res) e->be->fold_into(b.ex->res->dev.get(), b.ex->par, b.ex->off_par, active, d);
+}
 }  // namespace
 
 extern "C" {
@@ -744,23 +916,7 @@ int gk_review_batch(gk_engine_t* e, const gk_obj* objs, size_t n, const char* ep
     if (!rp->ev.viol.empty()) rp->ev.viol.resize(n * (size_t)W);
     if (!rp->ev.err.empty()) rp->ev.err.resize(n * (size_t)W);
     rp->ev.n = (uint32_t)n;
-    for (auto& v : rp->vio)
-      if (v.object >= n) {
-        const Child& ch = children[v.object - n];
-        v.object = ch.parent;
-        v.msg = ExpansionSystem::implied_by(ch.tmpl, v.msg);
-        if (!ch.action.empty()) v.action = ch.action;   // OverrideEnforcementAction (aggregate.go:47-58) sets EnforcementAction only: the scoped list stays
-      }
-    std::stable_sort(rp->vio.begin(), rp->vio.end(), [](const Violation& a, const Violation& b2) { return a.object < b2.object; });
-    if (rp->obj_errors.empty() && any_expand_err) rp->obj_errors.assign(total, std::string());
-    if (!rp->obj_errors.empty()) {
-      for (size_t k = 0; k < children.size(); ++k)
-        if (!rp->obj_errors[n + k].empty() && rp->obj_errors[children[k].parent].empty())
-          rp->obj_errors[children[k].parent] = ExpansionSystem::implied_by(children[k].tmpl, rp->obj_errors[n + k]);
-      rp->obj_errors.resize(n);
-      for (size_t i = 0; i < n && i < x.errors.size(); ++i)
-        if (!x.errors[i].empty() && rp->obj_errors[i].empty()) rp->obj_errors[i] = x.errors[i];
-    }
+    fold_results(rp->vio, rp->obj_errors, n, children, x.errors);
     const bool give_bits = !(flags & GK_F_NO_COPY_BACK);
     fill_result(out, rp, give_bits);
   });
@@ -770,9 +926,15 @@ int gk_batch_upload(gk_engine_t* e, const gk_obj* objs, size_t n, uint32_t flags
   if (!e || !outb || (!objs && n)) return GK_ERR_INVALID;
   if (stats) memset(stats, 0, sizeof *stats);
   return guard(err, [&]() {
+    const uint64_t xv = e->eng->expansion_version();   // (read before the flatten, as the excluder is)
     auto c = e->eng->compiled();
     ProgramLease lease(e, *c);
-    *outb = upload_batch(e, c, objs, n, flags, stats).release();
+    auto b = upload_batch(e, c, objs, n, flags, stats);
+    if (flags & GK_F_EXPAND) {
+      expand_batch(e, c, *b, xv, false);
+      if (stats) stats->alg_bytes = b->alg_bytes;
+    }
+    *outb = b.release();
   });
 }
 
@@ -780,7 +942,7 @@ int gk_batch_eval(gk_engine_t* e, gk_batch_t* b, const char* ep, uint32_t flags,
   if (!e || !b || !out) return GK_ERR_INVALID;
   memset(out, 0, sizeof *out);
   return guard(err, [&]() {
-    refuse_while_expanding(e);
+    require_expanded_or_none(e, *b);
     auto c = e->eng->compiled();
     require_current(e, *c, *b);
     ProgramLease lease(e, *c);
@@ -811,6 +973,7 @@ int gk_batch_eval_device_peers(gk_engine_t* e, gk_batch_t* b, const char* ep, co
   d.stream = stream;
   d.npeers = npeers;
   d.tot_stride = tot_stride;
+  d.rank = rank;
   for (uint32_t q = 0; q < npeers; ++q) {
     d.peer_viol[q] = peer_bases[q] + (uint64_t)rank * slot_i32 * 4;
     d.peer_tot[q] = peer_bases[q] + ((uint64_t)rank * slot_i32 + tot_off_i32) * 4;
@@ -823,9 +986,15 @@ int gk_batch_upload_blob(gk_engine_t* e, const char* buf, const uint64_t* offset
   if (!e || !outb || ((!buf || !offsets) && n)) return GK_ERR_INVALID;
   if (stats) memset(stats, 0, sizeof *stats);
   return guard(err, [&]() {
+    const uint64_t xv = e->eng->expansion_version();
     auto c = e->eng->compiled();
     ProgramLease lease(e, *c);
-    *outb = upload_blob(e, c, buf, offsets, n, source, flags, stats).release();
+    auto b = upload_blob(e, c, buf, offsets, n, source, flags, stats);
+    if (flags & GK_F_EXPAND) {
+      expand_batch(e, c, *b, xv, false);
+      if (stats) stats->alg_bytes = b->alg_bytes;
+    }
+    *outb = b.release();
   });
 }
 
@@ -834,12 +1003,14 @@ int gk_review_blob(gk_engine_t* e, const char* buf, const uint64_t* offsets, siz
   if (!e || !out || ((!buf || !offsets) && n)) return GK_ERR_INVALID;
   memset(out, 0, sizeof *out);
   return guard(err, [&]() {
-    refuse_while_expanding(e);
+    if (!(flags & GK_F_EXPAND)) refuse_while_expanding(e);
     gk_result stats;
     memset(&stats, 0, sizeof stats);
+    const uint64_t xv = e->eng->expansion_version();
     auto c = e->eng->compiled();
     ProgramLease lease(e, *c);
     auto b = upload_blob(e, c, buf, offsets, n, source, flags & ~(uint32_t)GK_F_KEEP_SOURCE, &stats);   // (the batch lives for this call only)
+    if (flags & GK_F_EXPAND) expand_batch(e, c, *b, xv, false);
     eval_batch(e, b.get(), ep, flags, out);
     out->flatten_ms = stats.flatten_ms;
     out->h2d_ms = stats.h2d_ms;
@@ -858,8 +1029,9 @@ int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err
   if (stats) memset(stats, 0, sizeof *stats);
   bool rebuilt = false;
   const int rc = guard(err, [&]() {
+    const uint64_t xv = e->eng->expansion_version();
     auto c = e->eng->compiled();
-    if (excluded_of(e, b->flags) == b->excluded && !stale_reason(e, *c, *b)) {
+    if (excluded_of(e, b->flags) == b->excluded && !stale_reason(e, *c, *b) && !expansion_stale(e, *b)) {
       if (stats) {
         stats->alg_bytes = b->alg_bytes;
         stats->n_objects = b->n;
@@ -869,13 +1041,18 @@ int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err
     }
     ProgramLease lease(e, *c);
     std::unique_ptr<gk_batch> nb;
+    const bool from_source = b->blob && b->source && device_ingest(*c, b->n);
     if (!b->blob) nb = upload_batch(e, c, b->objs.data(), b->objs.size(), b->flags, stats);
-    else if (b->source && device_ingest(*c, b->n)) nb = refresh_from_source(e, c, *b, stats);
+    else if (from_source) nb = refresh_from_source(e, c, *b, stats);
     else nb = upload_blob(e, c, b->blob, b->blob_off, b->n, b->blob_source, b->flags, stats);
     // the new columns replace the old ones; a kept source stays with the batch (a batch that had none may have gained one)
     if (!nb->source) {
       nb->source = std::move(b->source);
       nb->source_errors = std::move(b->source_errors);
+    }
+    if (b->flags & GK_F_EXPAND) {   // (expanded again whatever changed: the resultants' columns follow the constraint set too)
+      expand_batch(e, c, *nb, xv, from_source);
+      if (stats) stats->alg_bytes = nb->alg_bytes;
     }
     std::swap(*b, *nb);   // (the old columns are released with nb)
     rebuilt = true;

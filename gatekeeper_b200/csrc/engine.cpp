@@ -1983,6 +1983,15 @@ bool Engine::has_expansion() {
   std::shared_lock<std::shared_mutex> l(mu_);
   return !expansion_.empty();
 }
+uint64_t Engine::expansion_version() {
+  std::shared_lock<std::shared_mutex> l(mu_);
+  return expansion_.version();
+}
+bool Engine::expansion_selects(const std::string& g, const std::string& v, const std::string& k) {
+  if (g.empty() && v.empty() && k.empty()) return true;   // (System.Expand: "cannot expand resource ... with empty GVK")
+  std::shared_lock<std::shared_mutex> l(mu_);
+  return expansion_.generates_from(g, v, k);
+}
 void Engine::expand_object(const ObjIn& in, std::vector<Resultant>& out) {
   // the generator is the request's object -- the OLD object of a DELETE (getReqObject, pkg/webhook/policy.go:435-440,599-603)
   const bool del = in.operation && std::string(in.operation) == "DELETE";

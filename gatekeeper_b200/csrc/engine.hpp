@@ -197,6 +197,9 @@ class Engine {
   void add_expansion_template(const std::string& json);
   bool remove_expansion_template(const std::string& name);
   bool has_expansion();
+  uint64_t expansion_version();   // ExpansionSystem::version: an expanded batch is current while it is unchanged
+  // whether objects of (g, v, k) can have resultants: a stored template applies to it, or it is empty (expansion then fails)
+  bool expansion_selects(const std::string& g, const std::string& v, const std::string& k);
   std::vector<std::string> expansion_conflicts();   // System.GetConflicts: templates set aside as part of an expansion cycle, by name
   // the resultants of one review's object (empty when no template applies); throws std::runtime_error like System.Expand
   void expand_object(const ObjIn& in, std::vector<Resultant>& out);

@@ -73,6 +73,7 @@ void ExpansionSystem::upsert(const std::string& json) {
     throw std::runtime_error("ExpansionTemplate " + x.name + " generates GVK " + x.group + "/" + x.version + ", Kind=" + x.kind + ", but also applies to that same GVK");
   const std::string name = x.name;
   templates_[name] = std::move(x);
+  ++version_;
   recompute_conflicts();
   // db.upsert (db.go:222-245): the template is stored even when it closes a cycle -- it and the others on the cycle are set aside -- and the
   // caller is told (the reference's controller writes the error into the template's status)
@@ -81,6 +82,7 @@ void ExpansionSystem::upsert(const std::string& json) {
 
 bool ExpansionSystem::remove(const std::string& name) {
   const bool had = templates_.erase(name) != 0;
+  if (had) ++version_;
   recompute_conflicts();
   return had;
 }

@@ -3,6 +3,7 @@
 // pkg/audit/manager.go:733-765 and pkg/webhook/policy.go:610-646.  Mutators are outside this engine's scope (the mutation
 // system is not on the Client.Review path): resultants are reviewed as generated, unmutated.
 #pragma once
+#include <cstdint>
 #include <map>
 #include <string>
 #include <vector>
@@ -31,6 +32,14 @@ class ExpansionSystem {
   void upsert(const std::string& json);          // throws JsonError / std::runtime_error with ValidateTemplate's texts
   bool remove(const std::string& name);
   bool empty() const { return templates_.empty(); }
+  // bumped by every upsert that stores a template (one that closes a cycle included) and every remove that removes one
+  uint64_t version() const { return version_; }
+  // some stored template, set aside or not, applies to (g, v, k): an object of that kind may have resultants
+  bool generates_from(const std::string& g, const std::string& v, const std::string& k) const {
+    for (auto& t : templates_)
+      if (t.second.applies_to(g, v, k)) return true;
+    return false;
+  }
   std::vector<std::string> conflicts() const {   // System.GetConflicts -- system.go:81-83 (names, sorted)
     std::vector<std::string> out;
     for (auto& c : conflicted_)
@@ -49,6 +58,7 @@ class ExpansionSystem {
   std::vector<const ExpansionTemplate*> templates_for(const std::string& g, const std::string& v, const std::string& k) const;
   void recompute_conflicts();
   std::map<std::string, ExpansionTemplate> templates_;
+  uint64_t version_ = 0;
   std::map<std::string, bool> conflicted_;       // on a cycle of the generatedGVK -> applyTo graph: set aside (db.go hasConflicts)
 };
 

@@ -72,6 +72,11 @@ struct DevBatch {
   std::vector<uint32_t> cap;  // rows of the largest tile per scope (sizes the slot area of any netlist over this batch)
   std::vector<uint32_t> rows; // rows per scope in the batch, rows[0] = objects (sizes the generated kernel's export arrays)
   bool fork = false;          // a view made by fork_batch: arena and tiling belong to the batch it was forked from
+  // a resultant batch of an expanded batch (set_parents): its parents as a CSR, and the totals its own evaluations write
+  uint32_t* fold_par = nullptr;
+  uint32_t* fold_off = nullptr;
+  uint32_t fold_m = 0;
+  unsigned long long* fold_tot = nullptr;   // [2 * words * 32]
 };
 
 // ---- audit candidates (Backend::audit_candidates): rank the batch's identities, then select per constraint
@@ -222,6 +227,50 @@ __global__ void gk_sel_emit_kernel(const uint32_t* viol, const uint32_t* rank, c
     }
     cand[i] = out;
   }
+}
+
+// ---- expanded batches (Backend::select_generators, eval_expanded, fold_into)
+// 1 for every object whose apiVersion / kind hash was selected on the host (pick[slot] != 0), and for every object with hash 0
+__global__ void gk_gen_mark_kernel(const unsigned long long* gvk, uint32_t n, const unsigned long long* keys, const uint32_t* pick, uint32_t mask,
+                                   uint8_t* mark, uint32_t* idx) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const unsigned long long k = gvk[i];
+    uint8_t m = 1;
+    if (k)
+      for (uint32_t s = gk_gvk_slot(k, mask);; s = (s + 1) & mask)
+        if (keys[s] == k) {
+          m = pick[s] != 0;
+          break;
+        }
+    mark[i] = m;
+    idx[i] = i;
+  }
+}
+// one thread per parent with resultants (fold_core.h), the newly set bits counted per CTA in shared memory [2 * C], then one atomic per
+// CTA and constraint
+__global__ void __launch_bounds__(256) gk_fold_kernel(GkFoldArgs a) {
+  extern __shared__ uint32_t sh[];
+  const uint32_t C = a.nconstraints;
+  for (uint32_t c = threadIdx.x; c < 2 * C; c += blockDim.x) sh[c] = 0;
+  __syncthreads();
+  for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < a.m; j += gridDim.x * blockDim.x)
+    gk_fold_parent(a, j, [&](uint32_t c, uint32_t plane) {
+      if (c < C) atomicAdd(&sh[plane * C + c], 1u);
+    });
+  __syncthreads();
+  for (uint32_t c = threadIdx.x; c < C; c += blockDim.x) {
+    if (sh[c]) atomicAdd(a.totals + c, (unsigned long long)sh[c]);
+    if (sh[C + c]) atomicAdd(a.err_totals + c, (unsigned long long)sh[C + c]);
+  }
+}
+// the fused exchange: the folded totals replace the ones the evaluation published to every peer
+__global__ void gk_fold_publish_kernel(GkFoldArgs a) {
+  for (uint32_t c = threadIdx.x; c < a.nconstraints; c += blockDim.x)
+    for (uint32_t q = 0; q < a.npeers; ++q) {
+      a.peer_tot[q][c] = a.totals[c];
+      a.peer_tot[q][a.tot_stride + c] = a.err_totals[c];
+    }
+  __threadfence_system();
 }
 
 class CudaBackend : public Backend {
@@ -541,6 +590,9 @@ class CudaBackend : public Backend {
     dfree(db->err);
     if (!db->fork) dfree(db->d_tile_lo);
     if (!db->fork) dfree(db->gvk);
+    dfree(db->fold_par);
+    dfree(db->fold_off);
+    dfree(db->fold_tot);
     dfree(db->d_units);
     dfree(db->d_ops);
     dfree(db->d_pool);
@@ -965,6 +1017,38 @@ class CudaBackend : public Backend {
     if (!ks || ks->in.n != rq.n) throw BackendError{"device ingest: the kept source is of another page"};
     if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[launch] extraction of %u objects from the kept source: no copy, no tokeniser\n", ks->in.n);
     return extract(rq, [ks]() { return ks->in; }, ks->bytes, false, st, nullptr);
+  }
+
+  void source_bytes(void* source, const std::vector<uint32_t>& idx, std::string& bytes, std::vector<uint64_t>& off) override {
+    std::lock_guard<std::mutex> l(ingest_mu_);
+    CK(cudaSetDevice(device_));
+    auto* ks = static_cast<KeptSource*>(source);
+    if (!ks) throw BackendError{"kept source: none"};
+    std::vector<unsigned long long> ooff((size_t)ks->in.n + 1);
+    CK(cudaMemcpy(ooff.data(), ks->in.ooff, ooff.size() * 8, cudaMemcpyDeviceToHost));
+    std::vector<unsigned long long> spans;
+    off.assign(1, 0);
+    for (uint32_t i : idx) {
+      if (i >= ks->in.n) throw BackendError{"kept source: object index out of range"};
+      const unsigned long long len = ooff[i + 1] - ooff[i];
+      spans.insert(spans.end(), {ooff[i], (unsigned long long)off.back(), len});
+      off.push_back(off.back() + len);
+    }
+    bytes.assign((size_t)off.back(), '\0');
+    const uint32_t nspans = (uint32_t)(spans.size() / 3);
+    if (!nspans || bytes.empty()) return;
+    unsigned long long* d_spans = nullptr;
+    uint8_t* d_out = nullptr;
+    dmalloc(&d_spans, spans.size() * 8);
+    dmalloc(&d_out, bytes.size());
+    CK(cudaMemcpyAsync(d_spans, spans.data(), spans.size() * 8, cudaMemcpyHostToDevice, stream_));
+    gk_gather_kernel<<<std::min<uint32_t>(nspans, 4096u), 128, 0, stream_>>>(d_out, ks->in.blob, d_spans, nspans);
+    ++launches_;
+    CK(cudaMemcpyAsync(&bytes[0], d_out, bytes.size(), cudaMemcpyDeviceToHost, stream_));
+    dfree(d_spans);
+    dfree(d_out);
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
   }
 
   void release_source(void* source) override {
@@ -1731,6 +1815,228 @@ class CudaBackend : public Backend {
       p.peer_tot[q] = reinterpret_cast<unsigned long long*>(dst.peer_tot[q]);
     }
     fire(p, smem, st);
+  }
+
+  // Generator selection: the page's distinct apiVersion / kind hashes into a device table (as audit_candidates finds them), decided on
+  // the host from one object each, then every object marked and the marks compacted, in object order, into the index list.
+  void select_generators(void* b, const GvkOf& gvk_of, const GvkWanted& wanted, std::vector<uint32_t>& sel, uint32_t* kinds, float* device_ms) override {
+    auto* db = static_cast<DevBatch*>(b);
+    std::lock_guard<std::mutex> l(mu_);
+    CK(cudaSetDevice(device_));
+    const uint32_t n = db->n;
+    sel.clear();
+    if (kinds) *kinds = 0;
+    if (device_ms) *device_ms = 0.f;
+    if (!n) return;
+    if (!db->gvk) throw BackendError{"select generators: the batch holds no apiVersion / kind hashes"};
+    std::vector<void*> temps;
+    struct Free {
+      CudaBackend* be;
+      std::vector<void*>& t;
+      ~Free() {
+        for (void* p : t) be->dfree(p);
+      }
+    } free_temps{this, temps};
+    auto take = [&](size_t bytes) {
+      void* p = nullptr;
+      dmalloc(&p, bytes);
+      temps.push_back(p);
+      return p;
+    };
+    uint32_t cap = 1024;
+    while (cap < 2 * n) cap <<= 1;
+    const uint32_t mask = cap - 1, T = 256, grid = std::min<uint32_t>((n + T - 1) / T, (uint32_t)sms_ * 16);
+    auto* keys = static_cast<unsigned long long*>(take((size_t)cap * 8));
+    auto* rep = static_cast<uint32_t*>(take((size_t)cap * 4));
+    auto* d_cnt = static_cast<uint32_t*>(take(64));
+    auto* d_list = static_cast<uint32_t*>(take((size_t)2 * n * 4));
+    cudaEvent_t e0, e1, e2, e3;
+    for (cudaEvent_t* e : {&e0, &e1, &e2, &e3}) CK(cudaEventCreate(e));
+    struct Ev {
+      cudaEvent_t* e[4];
+      ~Ev() {
+        for (auto x : e) cudaEventDestroy(*x);
+      }
+    } ev_guard{{&e0, &e1, &e2, &e3}};
+    CK(cudaEventRecord(e0, stream_));
+    CK(cudaMemsetAsync(keys, 0, (size_t)cap * 8, stream_));
+    CK(cudaMemsetAsync(rep, 0xff, (size_t)cap * 4, stream_));
+    CK(cudaMemsetAsync(d_cnt, 0, 4, stream_));
+    gk_gvk_insert_kernel<<<grid, T, 0, stream_>>>(db->gvk, n, keys, rep, mask);
+    gk_gvk_collect_kernel<<<std::min<uint32_t>((cap + T - 1) / T, (uint32_t)sms_ * 16), T, 0, stream_>>>(keys, rep, cap, d_cnt, d_list);
+    CK(cudaEventRecord(e1, stream_));
+    uint32_t m = 0;
+    CK(cudaMemcpyAsync(&m, d_cnt, 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
+    std::vector<uint32_t> list((size_t)2 * m);
+    if (m) CK(cudaMemcpy(list.data(), d_list, list.size() * 4, cudaMemcpyDeviceToHost));
+    std::vector<uint32_t> pairs;   // (slot, 1) of every selected hash
+    for (uint32_t j = 0; j < m; ++j) {
+      std::string g, v, k;
+      gvk_of(list[2 * j + 1], g, v, k);
+      if (wanted(g, v, k)) pairs.insert(pairs.end(), {list[2 * j], 1u});
+    }
+    const uint32_t np = (uint32_t)(pairs.size() / 2);
+    auto* mark = static_cast<uint8_t*>(take(n));
+    auto* idx = static_cast<uint32_t*>(take((size_t)n * 4));
+    auto* d_sel = static_cast<uint32_t*>(take((size_t)n * 4));
+    CK(cudaEventRecord(e2, stream_));
+    CK(cudaMemsetAsync(rep, 0, (size_t)cap * 4, stream_));   // (rep is free again: now the pick flag per slot)
+    if (np) {
+      CK(cudaMemcpyAsync(d_list, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, stream_));
+      gk_gvk_assign_kernel<<<(np + T - 1) / T, T, 0, stream_>>>(d_list, np, rep);
+    }
+    gk_gen_mark_kernel<<<grid, T, 0, stream_>>>(db->gvk, n, keys, rep, mask, mark, idx);
+    size_t sel_bytes = 0;
+    CK(cub::DeviceSelect::Flagged(nullptr, sel_bytes, idx, mark, d_sel, d_cnt, (int64_t)n, stream_));
+    CK(cub::DeviceSelect::Flagged(take(sel_bytes), sel_bytes, idx, mark, d_sel, d_cnt, (int64_t)n, stream_));
+    CK(cudaEventRecord(e3, stream_));
+    uint32_t g = 0;
+    CK(cudaMemcpyAsync(&g, d_cnt, 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
+    sel.resize(g);
+    if (g) CK(cudaMemcpy(sel.data(), d_sel, (size_t)g * 4, cudaMemcpyDeviceToHost));
+    launches_ += 4 + (np ? 1 : 0);
+    if (kinds) *kinds = m;
+    float a = 0.f, c2 = 0.f;
+    cudaEventElapsedTime(&a, e0, e1);
+    cudaEventElapsedTime(&c2, e2, e3);
+    if (device_ms) *device_ms = a + c2;
+  }
+
+  void set_parents(void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off) override {
+    auto* r = static_cast<DevBatch*>(res);
+    std::lock_guard<std::mutex> l(mu_);
+    CK(cudaSetDevice(device_));
+    if (off.size() != par.size() + 1) throw BackendError{"set_parents: the offsets must have one entry more than the parents"};
+    dfree(r->fold_par);
+    dfree(r->fold_off);
+    dfree(r->fold_tot);
+    r->fold_par = r->fold_off = nullptr;
+    r->fold_tot = nullptr;
+    r->fold_m = 0;
+    dmalloc(&r->fold_par, par.size() * 4);
+    dmalloc(&r->fold_off, off.size() * 4);
+    dmalloc(&r->fold_tot, (size_t)2 * r->words * 32 * 8);
+    if (!par.empty()) CK(cudaMemcpyAsync(r->fold_par, par.data(), par.size() * 4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(r->fold_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice, stream_));
+    CK(cudaStreamSynchronize(stream_));   // (the host vectors are the caller's)
+    r->fold_m = (uint32_t)par.size();
+  }
+
+  GkFoldArgs fold_args(const DevBatch& r) const {
+    GkFoldArgs a{};
+    a.par = r.fold_par;
+    a.off = r.fold_off;
+    a.m = r.fold_m;
+    a.words = r.words;
+    a.nconstraints = prog_.nconstraints;
+    a.cviol = r.viol;
+    a.cerr = r.err;
+    return a;
+  }
+  void launch_fold(const GkFoldArgs& a, cudaStream_t st) {
+    const uint32_t C = a.nconstraints;
+    if (!a.m || !C) return;
+    const size_t smem = (size_t)2 * C * 4;
+    if (smem > max_smem_) throw BackendError{"fold: too many constraints for one block's counters"};
+    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(gk_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const uint32_t T = 256, grid = std::max(1u, std::min<uint32_t>((a.m + T - 1) / T, (uint32_t)sms_ * 8));
+    gk_fold_kernel<<<grid, T, smem, st>>>(a);
+    CK(cudaGetLastError());
+    ++launches_;
+    if (a.npeers) {
+      gk_fold_publish_kernel<<<1, 256, 0, st>>>(a);
+      CK(cudaGetLastError());
+      ++launches_;
+    }
+  }
+
+  // eval() of the parents (their unfolded planes copied back into `own` when asked), eval() of the resultants into their own planes,
+  // then the fold into the parents' own planes (the device copy of the CSR, set_parents)
+  void eval_expanded(void* b, void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off, const std::vector<uint32_t>& active,
+                     EvalOut& out, bool copy_back, EvalOut* own, EvalOut* rout) override {
+    (void)par, (void)off;
+    eval(b, active, out, own != nullptr);
+    if (own) {
+      own->viol = std::move(out.viol);
+      own->err = std::move(out.err);
+      out.viol = BitPlane();
+      out.err = BitPlane();
+    }
+    EvalOut tmp;
+    EvalOut& r = rout ? *rout : tmp;
+    eval(res, active, r, rout != nullptr);
+    out.kernel_ms += r.kernel_ms;
+    fold_planes(b, res, out, copy_back);
+  }
+
+  // the fold into `b`'s own planes after eval() of both; the newly set bits added to out's totals, the folded planes copied back
+  void fold_planes(void* b, void* res, EvalOut& out, bool copy_back) {
+    auto* db = static_cast<DevBatch*>(b);
+    auto* r = static_cast<DevBatch*>(res);
+    std::lock_guard<std::mutex> l(mu_);
+    CK(cudaSetDevice(device_));
+    const uint32_t C = prog_.nconstraints;
+    GkFoldArgs a = fold_args(*r);
+    a.sviol = a.dviol = db->viol;
+    a.serr = a.derr = db->err;
+    a.totals = r->fold_tot;
+    a.err_totals = r->fold_tot + C;
+    if (C) CK(cudaMemsetAsync(r->fold_tot, 0, (size_t)2 * C * 8, stream_));
+    CK(cudaEventRecord(ev0_, stream_));
+    launch_fold(a, stream_);
+    CK(cudaEventRecord(ev1_, stream_));
+    std::vector<unsigned long long> t(2 * (size_t)C);
+    if (C) CK(cudaMemcpyAsync(t.data(), r->fold_tot, t.size() * 8, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, ev0_, ev1_));
+    out.kernel_ms += ms;
+    out.launches = launches_;
+    for (uint32_t c = 0; c < C && c < out.totals.size(); ++c) {
+      out.totals[c] += t[c];
+      out.err_totals[c] += t[C + c];
+    }
+    if (copy_back) {
+      out.viol.resize((size_t)db->n * db->words);
+      out.err.resize((size_t)db->n * db->words);
+      if (db->n) {
+        CK(cudaMemcpyAsync(out.viol.data(), db->viol, out.viol.size() * 4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaMemcpyAsync(out.err.data(), db->err, out.err.size() * 4, cudaMemcpyDeviceToHost, stream_));
+        CK(cudaStreamSynchronize(stream_));
+      }
+    }
+  }
+
+  void fold_into(void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off, const std::vector<uint32_t>& active,
+                 const DevOutPtrs& dst) override {
+    (void)par, (void)off;   // (the device copy of set_parents)
+    auto* r = static_cast<DevBatch*>(res);
+    std::lock_guard<std::mutex> l(mu_);
+    CK(cudaSetDevice(device_));
+    if (dst.npeers > GK_MAX_PEERS || (dst.npeers && dst.rank >= dst.npeers)) throw BackendError{"fold: bad peer addressing"};
+    const uint32_t C = prog_.nconstraints;
+    cudaStream_t st = static_cast<cudaStream_t>(dst.stream);
+    // the resultants into their own planes (their totals are not the caller's)
+    size_t smem = 0;
+    KParams p = prepare(r, active, r->viol, r->err, r->fold_tot, r->fold_tot + std::max(C, 1u), st, &smem);
+    fire(p, smem, st);
+    GkFoldArgs a = fold_args(*r);
+    a.sviol = dst.npeers ? reinterpret_cast<const uint32_t*>(dst.peer_viol[dst.rank]) : static_cast<const uint32_t*>(dst.viol);
+    a.serr = a.derr = static_cast<uint32_t*>(dst.err);
+    a.dviol = dst.npeers ? nullptr : static_cast<uint32_t*>(dst.viol);
+    a.npeers = dst.npeers;
+    a.tot_stride = dst.tot_stride;
+    for (uint32_t q = 0; q < dst.npeers; ++q) {
+      a.peer_viol[q] = reinterpret_cast<uint32_t*>(dst.peer_viol[q]);
+      a.peer_tot[q] = reinterpret_cast<unsigned long long*>(dst.peer_tot[q]);
+    }
+    a.totals = static_cast<unsigned long long*>(dst.totals);
+    a.err_totals = static_cast<unsigned long long*>(dst.err_totals);
+    launch_fold(a, st);
   }
 
  private:

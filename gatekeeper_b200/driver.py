@@ -26,6 +26,7 @@ SOURCE = {"": 0, None: 0, "Original": 1, "Generated": 2, "All": 3}
 
 F_BITMAP_ONLY, F_MATERIALIZE, F_NO_COPY_BACK = 0, 1, 2
 F_KEEP_SOURCE = 4
+F_EXPAND = 8          # expand the page's generator objects (ExpansionTemplates): an expanded batch
 F_PROCESS_AUDIT, F_PROCESS_WEBHOOK = 16, 32
 PROCESS_FLAG = {"": 0, None: 0, "audit": F_PROCESS_AUDIT, "webhook": F_PROCESS_WEBHOOK}
 
@@ -487,12 +488,15 @@ class Driver:
         return out
 
     # ---- resident batches (audit sweep / bench)
-    def upload(self, reviews: Iterable, process: str = ""):
+    def upload(self, reviews: Iterable, process: str = "", expand: bool = False):
+        """Flatten + upload review objects.  expand: an expanded batch (F_EXPAND) -- its generators' resultants are kept with it and
+        folded into their parents' rows by every evaluation."""
         arr, n, keep = self._marshal(reviews)
         h = C.c_void_p()
         stats = gk_result()
         err = C.c_char_p()
-        self._check(self._lib.gk_batch_upload(self._e, arr, n, PROCESS_FLAG.get(process, 0), C.byref(h), C.byref(stats), C.byref(err)), err)
+        flags = PROCESS_FLAG.get(process, 0) | (F_EXPAND if expand else 0)
+        self._check(self._lib.gk_batch_upload(self._e, arr, n, flags, C.byref(h), C.byref(stats), C.byref(err)), err)
         return ResidentBatch(self, h, (arr, keep), {"flatten_ms": stats.flatten_ms, "h2d_ms": stats.h2d_ms,
                                                     "h2d_bytes": stats.h2d_bytes, "alg_bytes": stats.alg_bytes})
 
@@ -507,13 +511,14 @@ class Driver:
         err = C.c_char_p()
         self._check(self._lib.gk_blob_prefetch(self._e, blob.buf, blob.offsets, len(blob), C.byref(err)), err)
 
-    def upload_blob(self, blob, source: str = "Original", process: str = "", keep_source: bool = False):
+    def upload_blob(self, blob, source: str = "Original", process: str = "", keep_source: bool = False, expand: bool = False):
         """Flatten + upload a page of objects held in one contiguous buffer (workloads.ObjectBlob).  keep_source: the batch keeps the
-        page's JSON and token tape on the device, so that ResidentBatch.refresh() re-extracts it without copying it again."""
+        page's JSON and token tape on the device, so that ResidentBatch.refresh() re-extracts it without copying it again.  expand: an
+        expanded batch (F_EXPAND), as for upload()."""
         h = C.c_void_p()
         stats = gk_result()
         err = C.c_char_p()
-        flags = PROCESS_FLAG.get(process, 0) | (F_KEEP_SOURCE if keep_source else 0)
+        flags = PROCESS_FLAG.get(process, 0) | (F_KEEP_SOURCE if keep_source else 0) | (F_EXPAND if expand else 0)
         self._check(self._lib.gk_batch_upload_blob(self._e, blob.buf, blob.offsets, len(blob), SOURCE.get(source, 4), flags, C.byref(h),
                                                    C.byref(stats), C.byref(err)), err)
         return ResidentBatch(self, h, blob, {"flatten_ms": stats.flatten_ms, "h2d_ms": stats.h2d_ms, "h2d_bytes": stats.h2d_bytes,
@@ -521,7 +526,8 @@ class Driver:
 
     def ReviewBlob(self, blob, enforcement_point: str = AUDIT_EP, flags: int = 0, source: str = "Original", with_results: bool = True,
                    zero_copy: bool = False) -> BatchResponse:
-        """End-to-end audit page: host JSON -> flatten -> H2D -> kernel -> D2H (+ optional message rendering)."""
+        """End-to-end audit page: host JSON -> flatten -> H2D -> kernel -> D2H (+ optional message rendering).  `flags` go to
+        gk_review_blob as they are: F_MATERIALIZE, F_EXPAND (expand the page's generators), F_PROCESS_*."""
         res = gk_result()
         err = C.c_char_p()
         keys = None

@@ -222,7 +222,8 @@ func (d *Driver) RemoveData(_ context.Context, _ string, path storage.Path) erro
 
 // UpsertExpansionTemplate / RemoveExpansionTemplate: the expansion system's templates (pkg/expansion/system.go:60-135).  With them
 // in place ReviewBatch reviews the resultants of every object in the same batch and folds their results onto the parent
-// ([Implied by <template>] prefix, enforcement-action override: pkg/expansion/aggregate.go:19-63).
+// ([Implied by <template>] prefix, enforcement-action override: pkg/expansion/aggregate.go:19-63).  The bitmap sweep entry points
+// (gk_batch_eval*, gk_review_blob), which this shim does not call, expand only a page uploaded with GK_F_EXPAND (gk_engine.h).
 func (d *Driver) UpsertExpansionTemplate(templateJSON []byte) error {
 	d.mux.Lock()
 	defer d.mux.Unlock()

@@ -47,6 +47,8 @@ enum {
   /* gk_batch_upload_blob: the batch keeps the page's device JSON, offsets and token tape until gk_batch_free, so that
    * gk_batch_refresh re-extracts its columns without copying or tokenising the page again (HBM cost: DESIGN.md section 5b) */
   GK_F_KEEP_SOURCE = 4,
+  /* gk_batch_upload, gk_batch_upload_blob, gk_review_blob: expand the page's generator objects (see gk_add_expansion_template) */
+  GK_F_EXPAND = 8,
   /* which caller's excluder applies at flatten time (gk_set_excluded_namespaces); neither bit = no excluder stage (gator) */
   GK_F_PROCESS_AUDIT = 16,   /* process.Audit   -- pkg/audit/manager.go:531-538,600 */
   GK_F_PROCESS_WEBHOOK = 32  /* process.Webhook -- pkg/webhook/policy.go:170-178 */
@@ -131,8 +133,19 @@ int gk_remove_constraint(gk_engine_t* e, const char* kind, const char* name);
  * audit loop (pkg/audit/manager.go:733-765) and the webhook (pkg/webhook/policy.go:610-646) do around Client.Review.  Mutators are
  * not applied (the mutation system is outside this engine).  gk_audit_add_batch does the same for a resident batch: the resultants'
  * results enter the run under the parent's identity, an object whose expansion fails contributes nothing and is an objectErrors entry.
- * The bitmap-only entry points (gk_batch_eval, gk_batch_eval_device(_peers), gk_review_blob) do not expand: while templates are
- * registered they fail with a text that says so, instead of returning rows in which the resultants' violations are missing. */
+ * The bitmap entry points (gk_batch_eval, gk_batch_eval_device(_peers), gk_review_blob) expand a page uploaded (or reviewed) with
+ * GK_F_EXPAND: an EXPANDED batch.  Its upload selects the page's generators on the device (the objects of an apiVersion / kind some
+ * stored template applies to), expands them on the host and uploads their resultants as a second resident batch, reviewed as
+ * Generated resources with the page's process flags.  Each evaluation evaluates the parents, then the resultants, then ORs every
+ * resultant's rows into its parent's rows on the device.  The planes, object_errors and (GK_F_MATERIALIZE) the violation list equal
+ * gk_review_batch's for the same objects; totals / err_totals are the column popcounts of the returned planes (parents with at least
+ * one result, own or implied -- gk_review_batch counts every resultant row).  gk_batch_size stays the number of parents; alg_bytes,
+ * kernel_ms and gpu_launches include the resultants and the fold.  The resultant planes belong to the batch: two device evaluations of
+ * one expanded batch must not overlap (order them on one stream).  An expanded batch is refused by the eval calls once templates have
+ * been added or removed since it was expanded ("ExpansionTemplates changed since the batch was expanded"); gk_batch_refresh expands
+ * it again (a GK_F_KEEP_SOURCE blob batch from its kept device copy).  gk_audit_add_batch(_ordered) ignores the resultants: it
+ * expands as for any batch.  Without GK_F_EXPAND these calls do not expand: while templates are registered they fail with a text
+ * that says so, instead of returning rows in which the resultants' violations are missing. */
 int gk_add_expansion_template(gk_engine_t* e, const char* json, size_t len, char** err);
 int gk_remove_expansion_template(gk_engine_t* e, const char* name);
 /* System.GetConflicts (pkg/expansion/system.go:81-83; db.go:62-70): the names of the stored ExpansionTemplates that are set aside
