@@ -61,6 +61,9 @@ struct DevBatch {
   // tiling (depends on the batch's row distribution and on the program's slot table)
   uint32_t* d_tile_lo = nullptr;
   uint32_t* d_units = nullptr;       // [2 * n] object ranges the specialised kernel hands to the interpreter (GkKParams::units): never more than objects
+  uint32_t* d_whole = nullptr;       // [ntiles + 1] the tiles handed over whole (GkKParams::whole), then the count of d_units
+  uint64_t planned = 0;              // the constraint-set version whose hand-over plan d_units / d_whole hold (0: none yet)
+  uint32_t nunits = 0;               // the plan's unit count
   // the netlist with every slot id replaced by the slot's word offset in this batch's shared-memory slot area
   GkOp* d_ops = nullptr;
   uint32_t* d_pool = nullptr;
@@ -314,6 +317,12 @@ class CudaBackend : public Backend {
     }
     CK(cudaEventCreate(&ev0_));
     CK(cudaEventCreate(&ev1_));
+    {
+      int lo = 0, hi = 0;
+      CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+      CK(cudaStreamCreateWithPriority(&side_stream_, cudaStreamNonBlocking, hi));   // fire(): the interpreter's units
+    }
+    CK(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
     cudaFuncAttributes fa;
     CK(cudaFuncGetAttributes(&fa, gk_eval_kernel));
     max_smem_ -= fa.sharedSizeBytes;   // the kernel's few static shared bytes come out of the same per-CTA budget
@@ -333,6 +342,8 @@ class CudaBackend : public Backend {
     if (pinned_) cudaFreeHost(pinned_);
     cudaEventDestroy(ev0_);
     cudaEventDestroy(ev1_);
+    cudaEventDestroy(ev_fork_);
+    cudaStreamDestroy(side_stream_);
     cudaStreamDestroy(stream_);
   }
   const char* name() const override { return "cuda-sm90a"; }
@@ -540,6 +551,7 @@ class CudaBackend : public Backend {
     push_small(db->d_outs, outs_r.data(), outs_r.size() * sizeof(GkOutEnt));
     db->words = std::max<uint32_t>(1, (uint32_t)((c.cons_match.size() + 31) / 32));
     dmalloc(&db->d_units, (size_t)db->n * 2 * 4);
+    dmalloc(&db->d_whole, ((size_t)db->ntiles + 1) * 4);
     dmalloc(&db->viol, (size_t)std::max(db->n, 1u) * db->words * 4);
     dmalloc(&db->err, (size_t)std::max(db->n, 1u) * db->words * 4);
     CK(cudaStreamSynchronize(stream_));
@@ -594,6 +606,7 @@ class CudaBackend : public Backend {
     dfree(db->fold_off);
     dfree(db->fold_tot);
     dfree(db->d_units);
+    dfree(db->d_whole);
     dfree(db->d_ops);
     dfree(db->d_pool);
     dfree(db->d_outs);
@@ -630,15 +643,16 @@ class CudaBackend : public Backend {
     p.npeers = 0;
     p.tot_stride = 0;
     p.done_ctr = reinterpret_cast<uint32_t*>(d_scalars_) + 4;   // zeroed with the error counter before every launch
+    p.done_target = 0;   // (set by fire())
     for (int q = 0; q < GK_MAX_PEERS; ++q) {
       p.peer_viol[q] = nullptr;
       p.peer_tot[q] = nullptr;
     }
     p.timing = nullptr;
     p.units = db->d_units;
-    p.unit_count = reinterpret_cast<uint32_t*>(d_scalars_) + 8;   // zeroed with the error counter before every launch
+    p.whole = db->d_whole;
+    p.unit_count = db->d_whole + db->ntiles;
     p.list_mode = 0;
-    p.pad_ = 0;
     spec_next_ = spec_ready(db->n);   // (an NVRTC run the first time: here, outside the timed region)
     if (spec_next_) {
       // The generated kernel stages the largest tile's rows in shared memory: 32 bits per row of a scope that has atoms (more when it
@@ -664,6 +678,20 @@ class CudaBackend : public Backend {
         if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[spec] export arrays: %zu bytes for %u objects\n", xb, db->n);
       }
       spec_rows_grid_ = spec_cur_->src.rows_blocks(db->rows, (uint32_t)spec_cur_->rows_threads);
+      // The hand-over plan depends on the batch's CSR offsets, which never change, and on the generated text: made by the first
+      // evaluation of the batch with this constraint set, here, and kept, with its unit count on the host.  (It reads every offset
+      // array the netlist uses: at config 2 about as long as the interpreter's units take, so planning on every evaluation would
+      // give back most of the overlap.)
+      if (spec_next_ && db->planned != spec_cur_->version && p.ntiles) {
+        CK(cudaMemsetAsync(p.unit_count, 0, 4, st));
+        void* args[] = {&p};
+        CK(cudaLaunchKernel(reinterpret_cast<const void*>(spec_cur_->plan_kern), dim3(p.ntiles), dim3(256), args, 0, st));
+        ++launches_;
+        CK(cudaMemcpyAsync(&db->nunits, p.unit_count, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        db->planned = spec_cur_->version;
+      }
+      spec_units_ = db->nunits;
     }
 #ifdef GK_PHASE_TIMING
     if (!d_timing_) CK(cudaMalloc(&d_timing_, (kMaxPhases + 2 + 16) * 16));
@@ -700,32 +728,50 @@ class CudaBackend : public Backend {
     if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[launch] %d CTAs/SM x %d threads, %zu B smem/CTA, %u tiles of %u objects\n", per_sm, kThreads, smem, p.ntiles, p.tile);
     uint32_t grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * per_sm)));
     last_kernel_ = "gk_eval_kernel";
-    if (spec_next_) {
-      // the kernel generated for this constraint set does the objects that fit its mask registers (all of them, normally); the
-      // interpreter behind it takes the object ranges it listed and, in the fused exchange, publishes the totals of both
-      SpecEntry& se = *spec_cur_;
-      uint32_t* xs = d_spec_x_;
-      void* args[] = {&p, &xs};
-      // the rows kernel evaluates every row of the batch into the export arrays, one thread per row
-      if (spec_rows_grid_) {
-        CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.rows_kern), dim3(spec_rows_grid_), dim3((unsigned)se.rows_threads), args, 0, st));
-        ++launches_;
-      }
-      // persistent CTAs, as many as are resident at once, walk the tiles with a grid stride: the per-CTA set-up (tables, enforcement
-      // mask) is paid once per CTA, and where two or more are resident one CTA's copy overlaps another's object walk.  (Launched as the
-      // rows kernel's programmatic dependent, so that this set-up overlaps the rows kernel's last blocks, it measured no faster.)
-      const uint32_t spec_grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * spec_per_sm_)));
-      CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.kern), dim3(spec_grid), dim3((unsigned)se.threads), args, spec_smem_, st));
+    if (!spec_next_) {
+      p.done_target = grid;
+      gk_eval_kernel<<<grid, kThreads, smem, st>>>(p);
+      CK(cudaGetLastError());
       ++launches_;
-      p.list_mode = 1;
-      last_kernel_ = "gk_spec_kernel";
-      // how many units there are is known only on the device: the persistent grid, each CTA striding over the list
-      grid = std::max(1u, std::min<uint32_t>(p.batch.n, (uint32_t)(sms_ * per_sm)));
+      return;
     }
-    gk_eval_kernel<<<grid, kThreads, smem, st>>>(p);
-    CK(cudaGetLastError());
+    // The kernel generated for this constraint set does the objects that fit its mask registers (all of them, normally); the
+    // interpreter does the object ranges the plan lists (prepare()), on a side stream while the rows kernel streams the batch:
+    //   st:    (memsets) fork -- rows kernel -- tile kernel -- wait(join)
+    //   side:         wait(fork) -- interpreter, list mode -- join
+    // The side stream has the higher priority, so that the interpreter's CTAs are placed at once instead of behind the rows
+    // kernel's pending blocks.  Neither grid waits for the other on the device: the two write disjoint words, add into the same
+    // totals, and in the fused exchange the last CTA of either publishes (done_target).  A batch without units launches no
+    // interpreter at all.
+    SpecEntry& se = *spec_cur_;
+    uint32_t* xs = d_spec_x_;
+    const uint32_t spec_grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * spec_per_sm_)));
+    // the interpreter's persistent grid, each CTA striding over the list
+    grid = std::max(1u, std::min<uint32_t>(p.batch.n, (uint32_t)(sms_ * per_sm)));
+    p.list_mode = 1;
+    p.done_target = spec_grid + (spec_units_ ? grid : 0u);
+    if (spec_units_) {
+      CK(cudaEventRecord(ev_fork_, st));
+      CK(cudaStreamWaitEvent(side_stream_, ev_fork_, 0));
+      gk_eval_kernel<<<grid, kThreads, smem, side_stream_>>>(p);
+      CK(cudaGetLastError());
+      ++launches_;
+      CK(cudaEventRecord(ev_fork_, side_stream_));   // (re-recorded as the join: the wait above already holds the fork)
+    }
+    void* args[] = {&p, &xs};
+    // the rows kernel evaluates every row of the batch into the export arrays, one thread per row
+    if (spec_rows_grid_) {
+      CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.rows_kern), dim3(spec_rows_grid_), dim3((unsigned)se.rows_threads), args, 0, st));
+      ++launches_;
+    }
+    // persistent CTAs, as many as are resident at once, walk the tiles with a grid stride: the per-CTA set-up (tables, enforcement
+    // mask) is paid once per CTA, and where two or more are resident one CTA's copy overlaps another's object walk.  (Launched as the
+    // rows kernel's programmatic dependent, so that this set-up overlaps the rows kernel's last blocks, it measured no faster.)
+    CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.kern), dim3(spec_grid), dim3((unsigned)se.threads), args, spec_smem_, st));
     ++launches_;
-    if (p.list_mode && getenv("GK_TRACE_LAUNCH")) {   // (a read-back, so only when tracing)
+    if (spec_units_) CK(cudaStreamWaitEvent(st, ev_fork_, 0));
+    last_kernel_ = "gk_spec_kernel";
+    if (getenv("GK_TRACE_LAUNCH")) {   // (a read-back, so only when tracing)
       uint32_t nu = 0;
       CK(cudaMemcpyAsync(&nu, p.unit_count, 4, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
@@ -749,6 +795,7 @@ class CudaBackend : public Backend {
     cudaLibrary_t lib = nullptr;
     cudaKernel_t kern = nullptr;        // gk_spec_kernel
     cudaKernel_t rows_kern = nullptr;   // gk_spec_rows_kernel
+    cudaKernel_t plan_kern = nullptr;   // gk_spec_plan_kernel
     int threads = 128, rows_threads = 256;
     size_t max_smem = 0;      // dynamic shared memory the kernel may be launched with (fixed part + the tile's staging area)
     double compile_ms = 0;
@@ -832,6 +879,7 @@ class CudaBackend : public Backend {
       CK(cudaLibraryLoadData(&se.lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0));
       CK(cudaLibraryGetKernel(&se.kern, se.lib, "gk_spec_kernel"));
       CK(cudaLibraryGetKernel(&se.rows_kern, se.lib, "gk_spec_rows_kernel"));
+      CK(cudaLibraryGetKernel(&se.plan_kern, se.lib, "gk_spec_plan_kernel"));
       se.threads = spec_threads_;
       se.rows_threads = spec_rows_threads_;
       cudaFuncAttributes fa;
@@ -2072,6 +2120,8 @@ class CudaBackend : public Backend {
   size_t max_smem_ = 0, sm_smem_ = 0;
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev0_ = nullptr, ev1_ = nullptr;
+  cudaStream_t side_stream_ = nullptr;   // fire(): the interpreter's units, beside the generated kernel
+  cudaEvent_t ev_fork_ = nullptr;
   std::mutex mu_;
   uint64_t version_ = 0, launches_ = 0;
   GkProgram prog_{};
@@ -2109,6 +2159,7 @@ class CudaBackend : public Backend {
   size_t spec_x_bytes_ = 0;
   uint32_t spec_rows_grid_ = 0;    // blocks of the next rows-kernel launch (set with spec_next_)
   bool spec_next_ = false;
+  uint32_t spec_units_ = 0;   // units the interpreter evaluates beside the next launch of the generated kernel (set with spec_next_)
   size_t spec_smem_ = 0;      // dynamic shared memory of the next launch of the generated kernel (set with spec_next_)
   int spec_per_sm_ = 1;       // its resident CTAs per SM at that size
   size_t optin_smem_ = 0;     // the device's per-CTA shared-memory limit

@@ -235,16 +235,40 @@ typedef struct {
   uint32_t npeers;
   uint32_t tot_stride;
   uint32_t* done_ctr;
+  uint32_t done_target;       // CTAs that count themselves in done_ctr: the last of them publishes (every CTA of both kernels
+                              // when the generated kernel and the interpreter's units run side by side)
   unsigned long long* timing; // GK_PHASE_TIMING builds: [kMaxPhases + 2][2] = (CTA cycles between barriers, summed warp busy cycles)
   // Hand-over list.  gk_spec_kernel keeps one mask word per netlist node and object, so an object may have at most 32 rows in a
-  // scope.  A tile with up to GK_HANDOVER_MAX such wide objects appends each of them as a unit (object, 1) and counts the rest
-  // itself; a tile with more appends itself whole, (first object, objects), and counts nothing.  gk_eval_kernel, launched behind
-  // it with list_mode = 1, evaluates exactly those units (and does the fused exchange's totals publication).
+  // scope.  gk_spec_plan_kernel finds those wide objects from the CSR offsets alone, before any row is evaluated: a tile with up
+  // to GK_HANDOVER_MAX of them appends each as a unit (object, 1); a tile with more appends itself whole, (first object,
+  // objects), and sets its whole flag.  gk_eval_kernel with list_mode = 1 evaluates exactly those units, while gk_spec_kernel
+  // does every other object and stores nothing for the units' objects.
   uint32_t* units;            // [2 * unit capacity]: (first object, objects) pairs, each inside one tile
   uint32_t* unit_count;
+  uint32_t* whole;            // [ntiles]: 1 = the tile is one unit of the list
   uint32_t list_mode;
-  uint32_t pad_;
 } GkKParams;
+#ifdef __CUDACC__
+// Fused exchange, the end of a CTA whose totals are in p.out: the last of the done_target CTAs to arrive (of whichever kernel)
+// sees every contribution and publishes the totals to all peers.  No CTA waits for another.  `s_last`: one word of shared memory.
+__device__ __forceinline__ void gk_publish_totals(const GkKParams& p, uint32_t nconstraints, volatile uint32_t* s_last) {
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) *s_last = atomicAdd(p.done_ctr, 1u) == p.done_target - 1u ? 1u : 0u;
+  __syncthreads();
+  if (*s_last) {
+    __threadfence();
+    for (uint32_t c = threadIdx.x; c < nconstraints; c += blockDim.x) {
+      const unsigned long long tv = atomicAdd(p.out.totals + c, 0ull), te = atomicAdd(p.out.err_totals + c, 0ull);
+      for (uint32_t q = 0; q < p.npeers; ++q) {
+        p.peer_tot[q][c] = tv;
+        p.peer_tot[q][p.tot_stride + c] = te;
+      }
+    }
+    __threadfence_system();
+  }
+}
+#endif
 // More wide objects than this in one tile hand the whole tile over.  A one-object unit pays the interpreter's per-phase barriers and
 // latencies for 1/512 of a tile's work.  Measured on an H100 over 1 M config-2 Pods with a wide object every 512 / 256 / 128 / 100
 // objects (1, 2, 4, ~5 per tile), one by one against whole tiles: 0.58 / 0.89 / 1.43 / 1.72 ms against 1.35 / 1.43 / 1.48 / 1.47.

@@ -87,19 +87,14 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
 #pragma unroll
   for (uint32_t w = 0; w < GK_SPEC_W; ++w) tv[w] = te[w] = 0u;
   for (uint32_t t = blockIdx.x; t < p.ntiles; t += gridDim.x) {
+    // a tile handed over whole (gk_spec_plan_kernel) is the interpreter's: its words and its totals (uniform across the CTA)
+    if (__ldg(p.whole + t)) continue;
     const uint32_t obj0 = t * p.tile, nobj = min(p.tile, p.batch.n - obj0);
     // phase 1: the copy of the tile's exports and offsets, every thread of the CTA; phase 2: its objects, one per thread.  (The
     // barrier at the end of the tile keeps the next tile's copy from overwriting what the last objects of this one still read.)
     const uint32_t* tl = p.tile_lo + (size_t)t * NS;
     gk_spec_stage(p.batch, scopes, xs, tl, tl + NS, stg, threadIdx.x, blockDim.x);
     __syncthreads();
-    // An object with more rows in a scope than a mask register holds makes gk_spec_object() return true: it is listed for the
-    // interpreter (alone, or with its whole tile -- GK_HANDOVER_MAX), which evaluates it again and overwrites what this kernel stored
-    // for it; its totals are not counted here.  `big` takes one bit per pass over the tile (this thread's object is wide), shifted in.
-    uint32_t big = 0u;
-    uint32_t tvt[GK_SPEC_W], tet[GK_SPEC_W];
-#pragma unroll
-    for (uint32_t w = 0; w < GK_SPEC_W; ++w) tvt[w] = tet[w] = 0u;
 #ifdef GK_SPEC_X_STAGEONLY   /* (measurement only: the staging of every tile without the object walk; results differ) */
     for (uint32_t base = nobj; base < nobj; base += blockDim.x) {
 #else
@@ -109,73 +104,49 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
       uint32_t vw[GK_SPEC_W], ew[GK_SPEC_W];
 #pragma unroll
       for (uint32_t w = 0; w < GK_SPEC_W; ++w) vw[w] = ew[w] = 0u;
-      big <<= 1;
       if (o < nobj) {
-        if (gk_spec_object(p.batch, stg, p.prog.pool, p.prog.cbytes, actw, p.out, obj0 + o, o, vw, ew)) {
-          big |= 1u;
+        // A wide object (gk_spec_object() returns true) is a unit of the interpreter's, which may be storing its words right now:
+        // nothing of it is stored here, and it is out of the totals.
+        const bool wide = gk_spec_object(p.batch, stg, p.prog.pool, p.prog.cbytes, actw, p.out, obj0 + o, o, vw, ew);
+        if (wide) {
 #pragma unroll
-          for (uint32_t w = 0; w < GK_SPEC_W; ++w) vw[w] = ew[w] = 0u;   // (out of the tile's totals; the interpreter stores its words)
-        }
-        const size_t at = (size_t)(obj0 + o) * GK_SPEC_W;
-#if GK_SPEC_W == 2
-        const uint2 v2 = make_uint2(vw[0], vw[1]);
-        if (p.npeers) {
-          for (uint32_t q = 0; q < p.npeers; ++q) *reinterpret_cast<uint2*>(p.peer_viol[q] + at) = v2;   // this rank is one of the peers
+          for (uint32_t w = 0; w < GK_SPEC_W; ++w) vw[w] = ew[w] = 0u;
         } else {
-          *reinterpret_cast<uint2*>(p.out.viol + at) = v2;
-        }
-        *reinterpret_cast<uint2*>(p.out.err + at) = make_uint2(ew[0], ew[1]);
+          const size_t at = (size_t)(obj0 + o) * GK_SPEC_W;
+#if GK_SPEC_W == 2
+          const uint2 v2 = make_uint2(vw[0], vw[1]);
+          if (p.npeers) {
+            for (uint32_t q = 0; q < p.npeers; ++q) *reinterpret_cast<uint2*>(p.peer_viol[q] + at) = v2;   // this rank is one of the peers
+          } else {
+            *reinterpret_cast<uint2*>(p.out.viol + at) = v2;
+          }
+          *reinterpret_cast<uint2*>(p.out.err + at) = make_uint2(ew[0], ew[1]);
 #else
 #pragma unroll
-        for (uint32_t w = 0; w < GK_SPEC_W; ++w) {
-          if (p.npeers) {
-            for (uint32_t q = 0; q < p.npeers; ++q) p.peer_viol[q][at + w] = vw[w];
-          } else {
-            p.out.viol[at + w] = vw[w];
+          for (uint32_t w = 0; w < GK_SPEC_W; ++w) {
+            if (p.npeers) {
+              for (uint32_t q = 0; q < p.npeers; ++q) p.peer_viol[q][at + w] = vw[w];
+            } else {
+              p.out.viol[at + w] = vw[w];
+            }
+            p.out.err[at + w] = ew[w];
           }
-          p.out.err[at + w] = ew[w];
-        }
 #endif
+        }
       }
       // totals: after the transpose lane c holds the bit of constraint (32 w + c) for the warp's 32 objects
       uint32_t anye = 0u;
 #pragma unroll
       for (uint32_t w = 0; w < GK_SPEC_W; ++w) {
-        tvt[w] += (uint32_t)__popc(gk_tr32(vw[w], lane));
+        tv[w] += (uint32_t)__popc(gk_tr32(vw[w], lane));
         anye |= ew[w];
       }
       if (__any_sync(0xffffffffu, anye != 0u)) {
 #pragma unroll
-        for (uint32_t w = 0; w < GK_SPEC_W; ++w) tet[w] += (uint32_t)__popc(gk_tr32(ew[w], lane));
+        for (uint32_t w = 0; w < GK_SPEC_W; ++w) te[w] += (uint32_t)__popc(gk_tr32(ew[w], lane));
       }
     }
-    bool whole = false;
-    if (__syncthreads_or(big)) {   // (uniform: every thread makes the same passes, so the counts below are exact)
-      uint32_t nbig = 0u;
-      const uint32_t last = (nobj - 1u) / blockDim.x;   // bit k of `big`: this thread's object of pass last - k
-      for (uint32_t k = 0; k <= last; ++k) nbig += (uint32_t)__syncthreads_count((big >> k) & 1u);
-      whole = nbig > GK_HANDOVER_MAX;
-      if (whole) {
-        if (threadIdx.x == 0) {
-          const uint32_t u = atomicAdd(p.unit_count, 1u);
-          p.units[2 * u] = obj0;
-          p.units[2 * u + 1] = nobj;
-        }
-      } else if (big) {
-        uint32_t u = atomicAdd(p.unit_count, (uint32_t)__popc(big));
-        for (; big; big &= big - 1u, ++u) {
-          p.units[2 * u] = obj0 + (last - ((uint32_t)__ffs(big) - 1u)) * blockDim.x + threadIdx.x;
-          p.units[2 * u + 1] = 1u;
-        }
-      }
-    }
-    if (!whole) {
-#pragma unroll
-      for (uint32_t w = 0; w < GK_SPEC_W; ++w) {
-        tv[w] += tvt[w];
-        te[w] += tet[w];
-      }
-    }
+    __syncthreads();
   }
 #pragma unroll
   for (uint32_t w = 0; w < GK_SPEC_W; ++w) {
@@ -187,13 +158,71 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
     if (s_tot[c]) atomicAdd(p.out.totals + c, (unsigned long long)s_tot[c]);
     if (s_err[c]) atomicAdd(p.out.err_totals + c, (unsigned long long)s_err[c]);
   }
+  if (p.npeers) gk_publish_totals(p, GK_SPEC_C, act);   // (act is free by now)
+}
+
+// The hand-over plan, before any row is evaluated: one CTA per tile finds the tile's wide objects from the CSR offsets
+// (gk_spec_wide) and lists them for the interpreter -- each alone, or the whole tile when it has more than GK_HANDOVER_MAX
+// (gk_spec_tile_whole) -- and sets the tile's whole flag, which gk_spec_kernel reads.
+extern "C" __global__ void gk_spec_plan_kernel(const __grid_constant__ GkKParams p) {
+  const uint32_t t = blockIdx.x, obj0 = t * p.tile, nobj = min(p.tile, p.batch.n - obj0);
+  uint32_t nwide = 0u;
+  for (uint32_t base = 0; base < nobj; base += blockDim.x) {
+    const uint32_t o = base + threadIdx.x;
+    nwide += (uint32_t)__syncthreads_count(o < nobj && gk_spec_wide(p.batch.scopes, obj0 + o));
+  }
+  const bool whole = gk_spec_tile_whole(nwide);
+  if (threadIdx.x == 0) {
+    p.whole[t] = whole ? 1u : 0u;
+    if (whole) {
+      const uint32_t u = atomicAdd(p.unit_count, 1u);
+      p.units[2 * u] = obj0;
+      p.units[2 * u + 1] = nobj;
+    }
+  }
+  if (nwide && !whole)
+    for (uint32_t o = threadIdx.x; o < nobj; o += blockDim.x)
+      if (gk_spec_wide(p.batch.scopes, obj0 + o)) {
+        const uint32_t u = atomicAdd(p.unit_count, 1u);
+        p.units[2 * u] = obj0 + o;
+        p.units[2 * u + 1] = 1u;
+      }
 }
 #else
 #include <vector>
+#include <cstdio>
+#include <cstdlib>
+#include <string>
+// TEST-ONLY host build: the hand-over plan of gk_spec_plan_kernel for tiles of `tile` objects, tile after tile and a tile's
+// objects in order (the kernel appends them in any order).  Fills units (capacity: 2 per object) and whole (one per tile); returns
+// the units.
+#ifndef GK_SPEC_HOST_PLAN_TILE
+#define GK_SPEC_HOST_PLAN_TILE 512u   /* the device's tile (tile_kernel.cuh GK_TILE) */
+#endif
+static uint32_t gk_spec_host_plan(const GkBatch& B, uint32_t tile, std::vector<uint32_t>& units, std::vector<uint32_t>& whole) {
+  units.clear();
+  whole.assign((B.n + tile - 1u) / tile, 0u);
+  for (uint32_t t = 0; t < whole.size(); ++t) {
+    const uint32_t obj0 = t * tile, nobj = B.n - obj0 < tile ? B.n - obj0 : tile;
+    uint32_t nwide = 0u;
+    for (uint32_t o = 0; o < nobj; ++o) nwide += gk_spec_wide(B.scopes, obj0 + o) ? 1u : 0u;
+    whole[t] = gk_spec_tile_whole(nwide) ? 1u : 0u;
+    if (whole[t]) {
+      units.insert(units.end(), {obj0, nobj});
+    } else {
+      for (uint32_t o = 0; o < nobj; ++o)
+        if (gk_spec_wide(B.scopes, obj0 + o)) units.insert(units.end(), {obj0 + o, 1u});
+    }
+  }
+  return (uint32_t)(units.size() / 2);
+}
 // TEST-ONLY host build (tests/_hostemu, GK_SPEC_CHECK=1): one object; returns 1 when the object does not fit the mask registers.
 // The rows of the object's tile (GK_SPEC_HOST_TILE objects; its rows found through the CSR offsets) are evaluated by the same
 // gk_spec_row_<g>() the rows kernel runs into a poisoned export buffer, which the same gk_spec_stage() the tile kernel runs copies
 // with three "threads" striding over it; both again only when `obj` leaves the tile (or starts it again).
+// The objects are checked in order: at the last one the hand-over plan of the batch is made, and every object the plan's test
+// (gk_spec_wide) decides otherwise than the object walk did is counted.  GK_SPEC_TRACE=1 prints the plan and that count:
+//   [spec plan] tiles of T: U units: <first object>+<objects> ...; whole tiles: <tile> ...; disagreements: D
 #ifndef GK_SPEC_HOST_TILE
 #define GK_SPEC_HOST_TILE 96u
 #endif
@@ -206,6 +235,7 @@ extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint
     const void* flags = nullptr;
     uint32_t n = 0, t = 0xffffffffu;
     std::vector<uint32_t> lo, hi, stg, x;
+    std::vector<uint8_t> walk_wide;   // what gk_spec_object() returned, per object of the batch so far
   };
   static thread_local Tile k;
   const GkBatch& B = p->batch;
@@ -224,7 +254,25 @@ extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint
     k.n = B.n;
     k.t = t;
   }
-  return gk_spec_object(B, k.stg.data(), p->prog.pool, p->prog.cbytes, actw, p->out, obj, obj - t * T, vw, ew) ? 1 : 0;
+  const int wide = gk_spec_object(B, k.stg.data(), p->prog.pool, p->prog.cbytes, actw, p->out, obj, obj - t * T, vw, ew) ? 1 : 0;
+  if (obj == 0u) k.walk_wide.assign(B.n, 2u);   // (2: not walked)
+  if (obj < k.walk_wide.size()) k.walk_wide[obj] = (uint8_t)wide;
+  if (obj + 1u == B.n && k.walk_wide.size() == B.n) {
+    uint32_t disagree = 0u;
+    for (uint32_t o = 0; o < B.n; ++o) disagree += k.walk_wide[o] != (gk_spec_wide(B.scopes, o) ? 1u : 0u);
+    std::vector<uint32_t> units, whole;
+    const uint32_t nu = gk_spec_host_plan(B, GK_SPEC_HOST_PLAN_TILE, units, whole);
+    if (getenv("GK_SPEC_TRACE")) {
+      std::string line = "[spec plan] tiles of " + std::to_string(GK_SPEC_HOST_PLAN_TILE) + ": " + std::to_string(nu) + " units:";
+      for (uint32_t u = 0; u < nu; ++u) line += " " + std::to_string(units[2 * u]) + "+" + std::to_string(units[2 * u + 1]);
+      line += "; whole tiles:";
+      for (uint32_t w = 0; w < whole.size(); ++w)
+        if (whole[w]) line += " " + std::to_string(w);
+      line += "; disagreements: " + std::to_string(disagree);
+      fprintf(stderr, "%s\n", line.c_str());
+    }
+  }
+  return wide;
 }
 #endif
 )GKSRC";
@@ -1024,21 +1072,38 @@ struct uint4 { uint32_t x, y, z, w; };
     o << "  }\n";
   }
   o << "  GK_SPEC_CP_WAIT();\n}\n";
-  // ---- phase 2, gk_spec_object(): one thread per object, from shared memory.  Returns true when the object has more rows in some
-  // scope than a mask holds: its words are then meaningless (the caller hands the tile to the interpreter, which stores them again;
-  // a matcher error may be listed twice, with the same code).  `o` is the object's index in the tile, `obj` its index in the batch.
+  // ---- which objects are WIDE: more rows in some used nested scope than a mask register holds.  The object's row range in scope s,
+  // [lo<s>, hi<s>), from its parent's through s's CSR offsets, read by `off(s, row)`.  A scope with more rows than a mask holds
+  // counts as EMPTY from there on and raises `big`: no branch.  gk_spec_object() reads the tile's staged offsets, gk_spec_wide()
+  // (the hand-over plan) the batch's own: one text, so that the two decide every object alike.
+  auto scope_extent = [&](uint32_t s, const std::function<std::string(const std::string&)>& off) {
+    const uint32_t P = parent_of(s);
+    o << "  const uint32_t lo" << s << " = " << off("lo" + std::to_string(P)) << ", r" << s << " = " << off("hi" + std::to_string(P)) << " - lo" << s << ";\n";
+    o << "  const uint32_t n" << s << " = r" << s << " > GK_SPEC_MASK_ROWS ? 0u : r" << s << ", hi" << s << " = lo" << s << " + n" << s << ";\n";
+    o << "  big = big || r" << s << " > GK_SPEC_MASK_ROWS;\n";
+  };
+  o << "\n#define GK_SPEC_MASK_ROWS 32u\n";
+  o << "GK_SPEC_FN bool gk_spec_wide(const GkScope* __restrict__ scopes, const uint32_t obj) {\n";
+  o << "  const uint32_t lo0 = obj, hi0 = obj + 1u;\n  (void)scopes; (void)lo0; (void)hi0;\n  bool big = false;\n";
+  for (uint32_t s : nested) {
+    scope_extent(s, [&](const std::string& row) { return "GK_SPEC_LD(scopes[" + std::to_string(s) + "].off + " + row + ")"; });
+    o << "  (void)hi" << s << ";\n";
+  }
+  o << "  return big;\n}\n";
+  o << "// the hand-over rule per tile: a tile with more wide objects than this goes to the interpreter whole (program.h)\n";
+  o << "GK_SPEC_FN bool gk_spec_tile_whole(const uint32_t nwide) { return nwide > GK_HANDOVER_MAX; }\n";
+  // ---- phase 2, gk_spec_object(): one thread per object, from shared memory.  Returns true when the object is wide: its words are
+  // then meaningless (the interpreter evaluates it, gk_spec_wide() having listed it; a matcher error may be listed twice, with the
+  // same code).  `o` is the object's index in the tile, `obj` its index in the batch.
   o << "\nGK_SPEC_FN bool gk_spec_object(const GkBatch& B, const uint32_t* stg, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes,\n"
        "                               const uint32_t* actw, const GkOut& out, const uint32_t obj, const uint32_t o, uint32_t* vw, uint32_t* ew) {\n";
   o << "  const uint32_t lo0 = o, hi0 = o + 1u, n0 = 1u, f0 = 1u;\n  (void)lo0; (void)hi0; (void)n0; (void)f0; (void)out; (void)pool; (void)cbytes; (void)stg;\n";
   o << "  bool big = false;\n";
   for (size_t j = 0; j < nested.size(); ++j) {
-    const uint32_t s = nested[j], P = parent_of(s);
+    const uint32_t s = nested[j];
     o << "  const uint32_t* __restrict__ q" << s << " = stg + stg[" << NG + j << "];\n";
-    // (a scope with more rows than a mask holds counts as EMPTY from here on and raises `big`: no branch)
-    o << "  const uint32_t lo" << s << " = q" << s << "[lo" << P << "], r" << s << " = q" << s << "[hi" << P << "] - lo" << s << ";\n";
-    o << "  const uint32_t n" << s << " = r" << s << " > 32u ? 0u : r" << s << ", hi" << s << " = lo" << s << " + n" << s << ";\n";
-    o << "  const uint32_t f" << s << " = n" << s << " >= 32u ? 0xffffffffu : ((1u << n" << s << ") - 1u);\n  (void)hi" << s << "; (void)f" << s << ";\n  big = big || r" << s
-      << " > 32u;\n";
+    scope_extent(s, [&](const std::string& row) { return "q" + std::to_string(s) + "[" + row + "]"; });
+    o << "  const uint32_t f" << s << " = n" << s << " >= 32u ? 0xffffffffu : ((1u << n" << s << ") - 1u);\n  (void)hi" << s << "; (void)f" << s << ";\n";
   }
   std::vector<uint8_t> group_done(groups.size(), 0), any_done(g.nvar, 0);
   auto emit_group = [&](size_t gi) {

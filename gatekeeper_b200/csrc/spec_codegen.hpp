@@ -8,7 +8,8 @@
 // (bit j = row j of THIS object in the node's scope), an export that only object-level EXISTS read one bit of the OR of the rows'
 // words, EXISTS a `!= 0`, the object-major bitmap words assembled in registers without a transpose.  NVRTC compiles that text for
 // sm_90a when the first large batch is evaluated (kernels.cu).  Objects with more than 32 rows in some scope do not fit the mask registers: they are
-// handed to the interpreter one by one, or with their whole tile when a tile holds more than GK_HANDOVER_MAX (GkKParams::units).
+// handed to the interpreter one by one, or with their whole tile when a tile holds more than GK_HANDOVER_MAX (GkKParams::units):
+// gk_spec_plan_kernel lists them from the CSR offsets before the rows are evaluated, and the interpreter runs beside the two kernels.
 #pragma once
 #include <string>
 #include <vector>
@@ -19,7 +20,7 @@ namespace gk {
 
 struct SpecSource {
   std::string src;        // one self-contained translation unit: program.h + vm_core.h + gk_spec_row_<g>() + gk_spec_rows_kernel + gk_spec_stage()
-                          // + gk_spec_object() + gk_spec_kernel
+                          // + gk_spec_wide() + gk_spec_object() + gk_spec_kernel + gk_spec_plan_kernel
   uint32_t words = 1;     // bitmap words per object
   size_t smem = 0;        // fixed dynamic shared memory of a launch (column / scope tables, enforcement-point mask, totals)
   size_t n_fast = 0, n_generic = 0;   // atoms emitted as immediates / as calls of the generic gk_atom()

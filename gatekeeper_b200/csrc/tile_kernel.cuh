@@ -387,7 +387,7 @@ __global__ void __launch_bounds__(kThreads, GK_MIN_CTAS) gk_eval_kernel(const KP
   uint32_t* pool = reinterpret_cast<uint32_t*>(smem + L.pool);
   uint8_t* cbytes = reinterpret_cast<uint8_t*>(smem + L.cbytes);
 
-  // list mode (behind gk_spec_kernel): only the object ranges that kernel handed over, usually none -- then nothing is staged
+  // list mode (beside gk_spec_kernel): only the object ranges gk_spec_plan_kernel listed; a CTA without one stages nothing
   const uint32_t nunits = p.list_mode ? *p.unit_count : p.ntiles;
   for (uint32_t i = threadIdx.x; i < C; i += blockDim.x) {
     s_tot[i] = 0;
@@ -701,26 +701,8 @@ __global__ void __launch_bounds__(kThreads, GK_MIN_CTAS) gk_eval_kernel(const KP
     if (s_tot[c]) atomicAdd(p.out.totals + c, (unsigned long long)s_tot[c]);
     if (s_err[c]) atomicAdd(p.out.err_totals + c, (unsigned long long)s_err[c]);
   }
-  if (p.npeers) {
-    // the last CTA to arrive sees every CTA's contribution and publishes the totals to all peers
-    // (the flag lives in the dynamic shared-memory area -- s_lo is free by now -- so the kernel keeps zero static shared bytes)
-    volatile uint32_t* s_last = s_lo;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) *s_last = atomicAdd(p.done_ctr, 1u) == gridDim.x - 1u ? 1u : 0u;
-    __syncthreads();
-    if (*s_last) {
-      __threadfence();
-      for (uint32_t c = threadIdx.x; c < C; c += blockDim.x) {
-        const unsigned long long tv = atomicAdd(p.out.totals + c, 0ull), te = atomicAdd(p.out.err_totals + c, 0ull);
-        for (uint32_t q = 0; q < p.npeers; ++q) {
-          p.peer_tot[q][c] = tv;
-          p.peer_tot[q][p.tot_stride + c] = te;
-        }
-      }
-      __threadfence_system();
-    }
-  }
+  // (the flag lives in the dynamic shared-memory area -- s_lo is free by now -- so the kernel keeps zero static shared bytes)
+  if (p.npeers) gk_publish_totals(p, C, s_lo);
 }
 
 }  // namespace gk
