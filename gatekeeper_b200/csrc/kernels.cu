@@ -64,6 +64,7 @@ struct DevBatch {
   uint32_t* d_whole = nullptr;       // [ntiles + 1] the tiles handed over whole (GkKParams::whole), then the count of d_units
   uint64_t planned = 0;              // the constraint-set version whose hand-over plan d_units / d_whole hold (0: none yet)
   uint32_t nunits = 0;               // the plan's unit count
+  uint64_t handed = 0;               // the objects those units cover
   // the netlist with every slot id replaced by the slot's word offset in this batch's shared-memory slot area
   GkOp* d_ops = nullptr;
   uint32_t* d_pool = nullptr;
@@ -655,9 +656,9 @@ class CudaBackend : public Backend {
     p.list_mode = 0;
     spec_next_ = spec_ready(db->n);   // (an NVRTC run the first time: here, outside the timed region)
     if (spec_next_) {
-      // The generated kernel stages the largest tile's rows in shared memory: 32 bits per row of a scope that has atoms (more when it
-      // has more than 32), where the interpreter holds one bit per row per live slot.  A scope with many rows in a tile and few atoms
-      // can therefore need more than the device allows while the interpreter fits: that batch is interpreted.
+      // The generated kernel stages the largest tile's rows in shared memory: one bit per row per export plane of a scope that has
+      // atoms, where the interpreter holds one bit per row per live slot.  A scope with many rows in a tile can therefore need more
+      // than the device allows while the interpreter fits: that batch is interpreted.
       spec_smem_ = spec_cur_->src.smem + spec_cur_->src.stage_bytes(db->cap);
       spec_next_ = spec_smem_ <= spec_cur_->max_smem;
       spec_per_sm_ = 0;   // resident CTAs per SM: the persistent grid of fire()
@@ -667,7 +668,27 @@ class CudaBackend : public Backend {
         spec_per_sm_ = spec_minb_;
       }
       spec_per_sm_ = std::max(1, spec_per_sm_);
-      // the export arrays: scratch rewritten by every evaluation, grown (never shrunk) outside the timed region
+      // The hand-over plan depends on the batch's CSR offsets, which never change, and on the generated text: made by the first
+      // evaluation of the batch with this constraint set, here, and kept, with its unit count and the objects they cover on the host.
+      // (It reads every offset array the netlist uses: at config 2 about as long as the interpreter's units take, so planning on
+      // every evaluation would give back most of the overlap.)
+      if (spec_next_ && db->planned != spec_cur_->version && p.ntiles) {
+        CK(cudaMemsetAsync(p.unit_count, 0, 4, st));
+        void* args[] = {&p};
+        CK(cudaLaunchKernel(reinterpret_cast<const void*>(spec_cur_->plan_kern), dim3(p.ntiles), dim3(256), args, 0, st));
+        ++launches_;
+        CK(cudaMemcpyAsync(&db->nunits, p.unit_count, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        std::vector<uint32_t> u((size_t)db->nunits * 2);
+        if (db->nunits) CK(cudaMemcpy(u.data(), p.units, u.size() * 4, cudaMemcpyDeviceToHost));
+        db->handed = 0;
+        for (uint32_t i = 0; i < db->nunits; ++i) db->handed += u[2 * i + 1];
+        db->planned = spec_cur_->version;
+      }
+      // A batch the plan hands over whole (every tile has more wide objects than GK_HANDOVER_MAX) is the interpreter's alone: the
+      // rows and tile kernels would evaluate every row for nothing.
+      if (spec_next_ && p.ntiles && db->handed >= db->n) spec_next_ = false;
+      // the export planes: scratch rewritten by every evaluation, grown (never shrunk) outside the timed region
       const size_t xb = spec_cur_->src.export_bytes(db->rows);
       if (spec_next_ && xb > spec_x_bytes_) {
         if (d_spec_x_) CK(cudaFree(d_spec_x_));
@@ -678,19 +699,6 @@ class CudaBackend : public Backend {
         if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[spec] export arrays: %zu bytes for %u objects\n", xb, db->n);
       }
       spec_rows_grid_ = spec_cur_->src.rows_blocks(db->rows, (uint32_t)spec_cur_->rows_threads);
-      // The hand-over plan depends on the batch's CSR offsets, which never change, and on the generated text: made by the first
-      // evaluation of the batch with this constraint set, here, and kept, with its unit count on the host.  (It reads every offset
-      // array the netlist uses: at config 2 about as long as the interpreter's units take, so planning on every evaluation would
-      // give back most of the overlap.)
-      if (spec_next_ && db->planned != spec_cur_->version && p.ntiles) {
-        CK(cudaMemsetAsync(p.unit_count, 0, 4, st));
-        void* args[] = {&p};
-        CK(cudaLaunchKernel(reinterpret_cast<const void*>(spec_cur_->plan_kern), dim3(p.ntiles), dim3(256), args, 0, st));
-        ++launches_;
-        CK(cudaMemcpyAsync(&db->nunits, p.unit_count, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        db->planned = spec_cur_->version;
-      }
       spec_units_ = db->nunits;
     }
 #ifdef GK_PHASE_TIMING

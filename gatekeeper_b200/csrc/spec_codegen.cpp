@@ -38,20 +38,6 @@ std::string hx(uint32_t v) {
 // the fixed part: launch wrapper (device) / per-object entry point (host test build)
 const char* kWrapper = R"GKSRC(
 #ifndef GK_SPEC_HOST
-__device__ __forceinline__ uint32_t gk_tr_step(uint32_t x, uint32_t lane, uint32_t j, uint32_t m) {
-  const uint32_t y = __shfl_xor_sync(0xffffffffu, x, j);
-  return (lane & j) ? ((x & ~m) | ((y & ~m) >> j)) : ((x & m) | ((y & m) << j));
-}
-// 32 x 32 bit transpose across the warp: lane i gives row i and receives column i
-__device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
-  x = gk_tr_step(x, lane, 16u, 0x0000ffffu);
-  x = gk_tr_step(x, lane, 8u, 0x00ff00ffu);
-  x = gk_tr_step(x, lane, 4u, 0x0f0f0f0fu);
-  x = gk_tr_step(x, lane, 2u, 0x33333333u);
-  x = gk_tr_step(x, lane, 1u, 0x55555555u);
-  return x;
-}
-
 extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_spec_kernel(const __grid_constant__ GkKParams p, const uint32_t* __restrict__ xs) {
   extern __shared__ uint4 gk_smem4[];
   unsigned char* smem = reinterpret_cast<unsigned char*>(gk_smem4);
@@ -255,7 +241,10 @@ extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint
     k.t = t;
   }
   const int wide = gk_spec_object(B, k.stg.data(), p->prog.pool, p->prog.cbytes, actw, p->out, obj, obj - t * T, vw, ew) ? 1 : 0;
-  if (obj == 0u) k.walk_wide.assign(B.n, 2u);   // (2: not walked)
+  if (obj == 0u) {
+    k.walk_wide.assign(B.n, 2u);   // (2: not walked)
+    if (getenv("GK_SPEC_TRACE")) gk_spec_trace_planes(B);
+  }
   if (obj < k.walk_wide.size()) k.walk_wide[obj] = (uint8_t)wide;
   if (obj + 1u == B.n && k.walk_wide.size() == B.n) {
     uint32_t disagree = 0u;
@@ -754,15 +743,32 @@ SpecSource spec_codegen(const Compiled& c) {
     }                                                                \
   }
 struct uint4 { uint32_t x, y, z, w; };
-#define GK_SPEC_CP4(d, s) (*(d) = *(s))
+#define GK_SPEC_CP16(d, s) (*(d) = *(s))
 #define GK_SPEC_CP_WAIT()
+static inline uint32_t gk_spec_funnel(uint32_t lo, uint32_t hi, uint32_t sh) { return (uint32_t)((((uint64_t)hi << 32) | lo) >> (sh & 31u)); }
+#define GK_SPEC_FUNNEL(lo, hi, sh) gk_spec_funnel(lo, hi, sh)
 #else
 #define GK_SPEC_FN __device__ __forceinline__
 #define GK_SPEC_LD(p) __ldg(p)      /* every array of a resident batch is read-only while it is evaluated */
 #define GK_SPEC_POPC(x) __popc(x)
-/* one 4-byte global -> shared copy in flight (the export slices are 4-byte aligned only); GK_SPEC_CP_WAIT() lands this thread's */
-#define GK_SPEC_CP4(d, s) asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((uint32_t)__cvta_generic_to_shared(d)), "l"(s) : "memory")
+/* one 16-byte global -> shared copy in flight (export planes and their regions are 16-byte aligned); GK_SPEC_CP_WAIT() lands this thread's */
+#define GK_SPEC_CP16(d, s) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"((uint32_t)__cvta_generic_to_shared(d)), "l"(s) : "memory")
 #define GK_SPEC_CP_WAIT() asm volatile("cp.async.wait_all;\n" ::: "memory")
+/* bits [sh, sh + 32) of the 64-bit word hi:lo */
+#define GK_SPEC_FUNNEL(lo, hi, sh) __funnelshift_r(lo, hi, sh)
+__device__ __forceinline__ uint32_t gk_tr_step(uint32_t x, uint32_t lane, uint32_t j, uint32_t m) {
+  const uint32_t y = __shfl_xor_sync(0xffffffffu, x, j);
+  return (lane & j) ? ((x & ~m) | ((y & ~m) >> j)) : ((x & m) | ((y & m) << j));
+}
+// 32 x 32 bit transpose across the warp: lane i gives row i and receives column i
+__device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
+  x = gk_tr_step(x, lane, 16u, 0x0000ffffu);
+  x = gk_tr_step(x, lane, 8u, 0x00ff00ffu);
+  x = gk_tr_step(x, lane, 4u, 0x0f0f0f0fu);
+  x = gk_tr_step(x, lane, 2u, 0x33333333u);
+  x = gk_tr_step(x, lane, 1u, 0x55555555u);
+  return x;
+}
 #define GK_SPEC_ERR(o, mid, code)                                    \
   {                                                                  \
     const uint32_t sl_ = atomicAdd(out.errcount, 1u);                \
@@ -856,8 +862,8 @@ struct uint4 { uint32_t x, y, z, w; };
   // or a gate of L whose inputs are row-local values and constants (and at least one of the former).  Phase 1 has every atom of a
   // row in a register, so it evaluates those gates there and stages only the EXPORTS: the row-local values that something else
   // reads -- an EXISTS, a broadcast, a gate with an input that is not row-local, a constraint's result.  An export that only
-  // object-level EXISTS read is in ANY form (phase 2 ORs the rows' staged words and tests one bit); every other export is in MASK
-  // form (phase 2 rebuilds the per-row mask, as it did for every atom before).  Constants, and gates of nothing but constants,
+  // object-level EXISTS read is in ANY form (phase 2 tests the object's window of its plane against 0); every other export is in MASK
+  // form (phase 2 takes the window as the per-row mask).  Constants, and gates of nothing but constants,
   // are literals in phase 1 and stay the nodes they were in phase 2.
   enum : uint8_t { kNotExported = 0, kAny = 1, kMask = 2 };
   std::vector<int> local(g.nvar, -1);      // variable -> the scope it is row-local in
@@ -922,53 +928,65 @@ struct uint4 { uint32_t x, y, z, w; };
   // per row loop: its exports (any form first), and the gates phase 1 evaluates for them, in netlist order
   std::vector<std::vector<uint32_t>> exports(groups.size()), gates(groups.size());
   std::vector<uint32_t> nany(groups.size(), 0);
-  std::vector<int> bit_of(g.nvar, -1);     // export -> its bit in the row's staged words
   for (uint8_t f : {kAny, kMask})
     for (uint32_t v = 0; v < g.nvar; ++v) {
       if (!live[v] || form[v] != f) continue;
       const size_t gi = (size_t)group_ix.at((uint32_t)local[v]);
-      bit_of[v] = (int)exports[gi].size();
       exports[gi].push_back(v);
       if (f == kAny) ++nany[gi];
     }
   for (uint32_t v = 0; v < g.nvar; ++v)
     if (live[v] && folded(v)) gates[(size_t)group_ix.at((uint32_t)local[v])].push_back(v);
   // ---- the rows, gk_spec_row_<g>() run by gk_spec_rows_kernel: one thread per row of a row loop's scope over the whole batch evaluates
-  // the loop's atoms and row-local gates (on a scope-0 row also the spec.match blocks, listing their errors) and stores the loop's
-  // exports as packed bits to the loop's EXPORT ARRAY in global memory, indexed by the row's batch index (ceil(exports / 32) words
-  // per row; bit k of word k / 32 = the loop's k-th export).  The arrays lie back to back in one scratch buffer, in row-loop order,
-  // each sized by its scope's rows in the batch (SpecSource::export_bytes).
-  // ---- the tile, gk_spec_stage(): the CTA copies the tile's slice of every export array, and of every used nested scope's CSR offsets
-  // (tile-relative), into shared memory.  The per-tile layout follows from the rows of every scope in the tile (tile_lo): a header
-  // of region offsets, then the regions.  SpecSource::stage lists them so the launch can size the area.
+  // the loop's atoms and row-local gates (on a scope-0 row also the spec.match blocks, listing their errors) and returns the loop's
+  // exports as packed bits (ceil(exports / 32) words; bit k of word k / 32 = the loop's k-th export).  The kernel stores them as BIT
+  // PLANES: a warp is 32 consecutive rows of one scope, aligned to 32, so a 32 x 32 bit transpose across the warp turns the warp's
+  // words into plane words, bit j = row 32 * blk + j.  Row loop g's planes are P<g> = its exports rounded up to 4 (the padding planes are 0), and
+  // word (blk, k) lies at X<g> + blk * P<g> + k: a block's planes are one 16-byte aligned run.  One guard block past the last keeps
+  // every window's high word (below) in bounds.  The loops' planes lie back to back in one scratch buffer, in row-loop order
+  // (SpecSource::export_bytes).
+  // ---- the tile, gk_spec_stage(): the CTA copies the tile's blocks of every row loop's planes (16-byte copies) and every used nested
+  // scope's CSR offsets (tile-relative) into shared memory.  The per-tile layout follows from the rows of every scope in the tile
+  // (tile_lo): a header of region offsets and of each row loop's first bit (b<s> & 31: the tile's first row of the scope within its
+  // block), then the regions.  SpecSource::stage lists them so the launch can size the area.
   std::vector<uint32_t> nested;   // used nested scopes: their offsets are staged
   for (size_t s = 1; s < NS; ++s)
     if (g.scope_used[s]) nested.push_back((uint32_t)s);
-  const uint32_t NG = (uint32_t)groups.size(), NR = NG + (uint32_t)nested.size(), data0 = (NR + 3u) & ~3u;
+  const uint32_t NG = (uint32_t)groups.size(), NR = NG + (uint32_t)nested.size(), data0 = (NR + NG + 3u) & ~3u;
   auto group_scope = [&](size_t gi) { return gscope[gi]; };
   auto group_words = [&](size_t gi) { return (uint32_t)((exports[gi].size() + 31) / 32); };
+  auto group_planes = [&](size_t gi) { return (uint32_t)((exports[gi].size() + 3) / 4 * 4); };
   for (size_t gi = 0; gi < NG; ++gi) {
-    out.stage.push_back({group_scope(gi), group_words(gi), 0u});
+    out.stage.push_back({group_scope(gi), group_planes(gi)});
     if (!groups[gi].empty())
       out.fold.push_back({group_scope(gi), (uint32_t)groups[gi].size(), (uint32_t)gates[gi].size(), nany[gi], (uint32_t)exports[gi].size() - nany[gi], group_words(gi)});
   }
-  for (uint32_t s : nested) out.stage.push_back({parent_of(s), 1u, 1u});
+  for (uint32_t s : nested) out.stage.push_back({parent_of(s), 0u});
   out.stage_hdr = data0;
   out.ngroups = NG;
-  std::ostringstream lay;   // the per-tile layout: b<s> / c<s> = first row / rows of scope s in the tile, R<g> / Q<s> = region offsets
+  // the per-tile layout: b<s> / c<s> = first row / rows of scope s in the tile, R<g> / Q<s> = region offsets.  Row loop g's region
+  // is ceil(c / 32) + 2 blocks, at least ((b & 31) + c) / 32 + 2: the ceil(((b & 31) + c) / 32) + 1 the copy fills (the tile's rows and
+  // the block after them) and, when (b & 31) + c is a multiple of 32, one more that only the window of an object with no rows there
+  // reads (masked to 0).
+  std::ostringstream lay;
   lay << "  const uint32_t b0 = GK_SPEC_LD(tlo), c0 = GK_SPEC_LD(thi) - b0;\n  (void)b0; (void)c0;\n";
   for (uint32_t s : nested)
     lay << "  const uint32_t b" << s << " = GK_SPEC_LD(tlo + " << s << "), c" << s << " = GK_SPEC_LD(thi + " << s << ") - b" << s << ";\n  (void)c" << s << ";\n";
   lay << "  uint32_t at = " << data0 << "u;\n";
-  for (size_t gi = 0; gi < NG; ++gi) lay << "  const uint32_t R" << gi << " = at;\n  at += c" << group_scope(gi) << " * " << group_words(gi) << "u;\n";
+  for (size_t gi = 0; gi < NG; ++gi) {
+    const std::string s = std::to_string(group_scope(gi));
+    lay << "  const uint32_t R" << gi << " = at;\n";
+    if (group_planes(gi)) lay << "  at += ((c" << s << " + 31u) / 32u + 2u) * " << group_planes(gi) << "u;\n";
+  }
   for (uint32_t s : nested) lay << "  const uint32_t Q" << s << " = at;\n  at += c" << parent_of(s) << " + 1u;\n";
-  // X<g> = the word offset of row loop g's export array in the scratch buffer; X<NG> = the buffer's words
+  // X<g> = the word offset of row loop g's planes in the scratch buffer; X<NG> = the buffer's words
   std::ostringstream xbase;
-  xbase << "  const size_t X0 = 0u;\n";
+  // (32-bit words: the planes are under one bit per row per export, and a scope's rows fit 32 bits)
+  xbase << "  const uint32_t X0 = 0u;\n";
   for (size_t gi = 0; gi < NG; ++gi) {
     const uint32_t s = group_scope(gi);
-    xbase << "  const size_t X" << gi + 1 << " = X" << gi << " + " << (s ? "(size_t)scopes[" + std::to_string(s) + "].rows" : std::string("(size_t)B.n")) << " * "
-          << group_words(gi) << "u;\n";
+    xbase << "  const uint32_t X" << gi + 1 << " = X" << gi << " + ((" << (s ? "scopes[" + std::to_string(s) + "].rows" : std::string("B.n")) << " + 31u) / 32u + 1u) * "
+          << group_planes(gi) << "u;\n";
   }
   xbase << "  (void)scopes;";
   for (size_t gi = 0; gi <= NG; ++gi) xbase << " (void)X" << gi << ";";
@@ -984,7 +1002,7 @@ struct uint4 { uint32_t x, y, z, w; };
       for (auto& kv : g.atoms[ai].need) need[kv.first] |= kv.second;
     o << "\n// atoms, row-local gates" << (s == 0 && !match_at[0].empty() ? ", spec.match blocks" : "") << " and exports of one row of scope " << s << " (row loop " << gi << ")\n";
     o << "GK_SPEC_FN void gk_spec_row_" << gi << "(const GkBatch& B, const GkColumn* cols, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes, const GkOut& out,\n"
-      << "                              const size_t row, uint32_t* __restrict__ xg) {\n  (void)B; (void)cols; (void)pool; (void)cbytes; (void)out;\n";
+      << "                              const size_t row, uint32_t* __restrict__ a) {\n  (void)B; (void)cols; (void)pool; (void)cbytes; (void)out; (void)a;\n";
     for (auto& kv : need) {
       const uint32_t ci = kv.first, enc = kv.second;
       const std::string K = std::to_string(ci);
@@ -1020,7 +1038,7 @@ struct uint4 { uint32_t x, y, z, w; };
     for (uint32_t w = 0; w < AW; ++w) o << (w ? ", a" : " a") << w << " = 0u";
     o << ";\n";
     for (size_t m = 0; m < exports[gi].size(); ++m) o << "  if (v" << exports[gi][m] << ") a" << m / 32 << " |= " << hx(1u << (m % 32)) << ";\n";
-    for (uint32_t w = 0; w < AW; ++w) o << "  xg[" << AW << "u * row + " << w << "u] = a" << w << ";\n";
+    for (uint32_t w = 0; w < AW; ++w) o << "  a[" << w << "] = a" << w << ";\n";
     o << "}\n";
   }
   o << "\n#ifdef GK_SPEC_HOST\n";
@@ -1030,36 +1048,71 @@ struct uint4 { uint32_t x, y, z, w; };
     o << "  tlo[" << s << "] = scopes[" << s << "].off[tlo[" << parent_of(s) << "]];\n  thi[" << s << "] = scopes[" << s << "].off[thi[" << parent_of(s) << "]];\n";
   o << "}\n";
   o << "static size_t gk_spec_export_words(const GkBatch& B) {\n  const GkScope* scopes = B.scopes;\n" << xbase.str() << "  return X" << NG << ";\n}\n";
-  // (the rows of the tile [tlo, thi) only: a copy that reads outside them finds the caller's poison)
-  o << "static void gk_spec_host_rows(const GkKParams* p, const uint32_t* tlo, const uint32_t* thi, uint32_t* xs) {\n  const GkBatch& B = p->batch;\n  const GkScope* scopes = B.scopes;\n"
-    << xbase.str();
-  for (size_t gi = 0; gi < NG; ++gi)
-    o << "  for (size_t row = tlo[" << group_scope(gi) << "]; row < thi[" << group_scope(gi) << "]; ++row) gk_spec_row_" << gi << "(B, B.cols, p->prog.pool, p->prog.cbytes, p->out, row, xs + X"
-      << gi << ");\n";
-  o << "}\n#else\n";
-  // one thread per row; blocks [first, first + ceil(rows / threads)) of the grid are row loop g's, so a block never mixes scopes
-  o << "extern \"C\" __global__ void __launch_bounds__(GK_SPEC_ROWS_THREADS, GK_SPEC_ROWS_MINB) gk_spec_rows_kernel(const __grid_constant__ GkKParams p, uint32_t* __restrict__ xs) {\n"
-    << "  const GkBatch& B = p.batch;\n  const GkScope* scopes = B.scopes;\n"
-    << xbase.str() << "  uint32_t blk = blockIdx.x;\n";
+  // GK_SPEC_TRACE: "[spec planes] loop <g>: scope <s>, <exports> exports, <rows> rows; ...; <words> export words" (once per batch)
+  o << "#include <cstdio>\nstatic void gk_spec_trace_planes(const GkBatch& B) {\n  fprintf(stderr, \"[spec planes]\");\n";
   for (size_t gi = 0; gi < NG; ++gi) {
     const uint32_t s = group_scope(gi);
-    o << "  {\n    const uint32_t nr = " << (s ? "scopes[" + std::to_string(s) + "].rows" : std::string("B.n")) << ", nb = (nr + GK_SPEC_ROWS_THREADS - 1u) / GK_SPEC_ROWS_THREADS;\n"
-      << "    if (blk < nb) {\n      const uint32_t row = blk * GK_SPEC_ROWS_THREADS + threadIdx.x;\n      if (row < nr) gk_spec_row_" << gi
-      << "(B, B.cols, p.prog.pool, p.prog.cbytes, p.out, row, xs + X" << gi << ");\n      return;\n    }\n    blk -= nb;\n  }\n";
+    o << "  fprintf(stderr, \" loop " << gi << ": scope " << s << ", " << exports[gi].size() << " exports, %u rows;\", " << (s ? "B.scopes[" + std::to_string(s) + "].rows" : std::string("B.n")) << ");\n";
   }
+  o << "  fprintf(stderr, \" %zu export words\\n\", gk_spec_export_words(B));\n}\n";
+  // (the rows of the tile [tlo, thi) only, and of those only their own bits of the plane words: a copy, or a window, that reads a row
+  // outside them finds the caller's poison)
+  o << "static void gk_spec_host_rows(const GkKParams* p, const uint32_t* tlo, const uint32_t* thi, uint32_t* xs) {\n  const GkBatch& B = p->batch;\n  const GkScope* scopes = B.scopes;\n"
+    << xbase.str();
+  for (size_t gi = 0; gi < NG; ++gi) {
+    const uint32_t s = group_scope(gi);
+    o << "  for (size_t row = tlo[" << s << "]; row < thi[" << s << "]; ++row) {\n    uint32_t a[" << std::max<uint32_t>(1, group_words(gi)) << "] = {0u};\n    gk_spec_row_" << gi
+      << "(B, B.cols, p->prog.pool, p->prog.cbytes, p->out, row, a);\n    uint32_t* x = xs + X" << gi << " + (row >> 5) * " << group_planes(gi) << "u;\n    const uint32_t r = 1u << (row & 31u);\n"
+      << "    for (uint32_t k = 0; k < " << exports[gi].size() << "u; ++k) x[k] = ((a[k >> 5] >> (k & 31u)) & 1u) ? (x[k] | r) : (x[k] & ~r);\n    (void)x; (void)r;\n  }\n";
+  }
+  o << "}\n#else\n";
+  // one thread per row; blocks [first, first + ceil(rows / threads)) of the grid are row loop g's, so a block never mixes scopes and
+  // a warp is one block of 32 rows.  Every lane reaches the transpose (a row past the scope's end contributes zeros); a warp past the
+  // scope's last block stores nothing.  The 32 x 32 transpose of word i (five shuffles, fewer instructions than a ballot per export
+  // from about eight exports up) leaves plane word 32 i + j of the block in lane j.
+  o << "static_assert(GK_SPEC_ROWS_THREADS % 32 == 0, \"a warp of gk_spec_rows_kernel is one block of 32 rows\");\n";
+  o << "extern \"C\" __global__ void __launch_bounds__(GK_SPEC_ROWS_THREADS, GK_SPEC_ROWS_MINB) gk_spec_rows_kernel(const __grid_constant__ GkKParams p, uint32_t* __restrict__ xs) {\n"
+    << "  const GkBatch& B = p.batch;\n  const GkScope* scopes = B.scopes;\n  const uint32_t lane = threadIdx.x & 31u;\n  (void)lane;\n"
+    << xbase.str() << "  uint32_t blk = blockIdx.x;\n";
+  // the block's row loop runs its row function and names its planes; the transpose and the store are one tail for every loop
+  uint32_t AWM = 1;
+  for (size_t gi = 0; gi < NG; ++gi) AWM = std::max(AWM, group_words(gi));
+  o << "  uint32_t nr = 0u, row = 0u, np = 0u";
+  for (uint32_t i = 0; i < AWM; ++i) o << ", a" << i << " = 0u";
+  o << ";\n  uint32_t xo = 0u;\n  do {\n";
+  for (size_t gi = 0; gi < NG; ++gi) {
+    const uint32_t s = group_scope(gi);
+    o << "    {\n      nr = " << (s ? "scopes[" + std::to_string(s) + "].rows" : std::string("B.n")) << ";\n      const uint32_t nb = (nr + GK_SPEC_ROWS_THREADS - 1u) / GK_SPEC_ROWS_THREADS;\n"
+      << "      if (blk < nb) {\n        row = blk * GK_SPEC_ROWS_THREADS + threadIdx.x;\n        if (row < nr) {\n          uint32_t w[" << std::max<uint32_t>(1, group_words(gi)) << "];\n          gk_spec_row_" << gi
+      << "(B, B.cols, p.prog.pool, p.prog.cbytes, p.out, row, w);\n";
+    for (uint32_t i = 0; i < group_words(gi); ++i) o << "          a" << i << " = w[" << i << "];\n";
+    o << "        }\n        np = " << group_planes(gi) << "u;\n        xo = X" << gi << ";\n        break;\n      }\n      blk -= nb;\n    }\n";
+  }
+  o << "    return;\n  } while (0);\n";
+  o << "  if ((row & ~31u) < nr) {\n    uint32_t* __restrict__ x = xs + xo + (size_t)(row >> 5) * np;\n";
+  for (uint32_t i = 0; i < AWM; ++i) {
+    o << "    " << (i ? "if (np > " + std::to_string(32 * i) + "u) " : std::string()) << "{\n      const uint32_t w = gk_tr32(a" << i << ", lane);\n      if (" << 32 * i
+      << "u + lane < np) x[" << 32 * i << "u + lane] = w;\n    }\n";
+  }
+  o << "  }\n";
   o << "}\n#endif\n";
-  // the copy: every 4-byte copy of the export slices in flight (cp.async) before the offsets' loads
+  // the copy: every 16-byte copy of the tile's plane blocks in flight (cp.async) before the offsets' loads
   o << "GK_SPEC_FN void gk_spec_stage(const GkBatch& B, const GkScope* scopes, const uint32_t* __restrict__ xs, const uint32_t* tlo, const uint32_t* thi, uint32_t* stg,\n"
        "                              const uint32_t tid, const uint32_t nthr) {\n  (void)B; (void)xs;\n";
   o << lay.str() << xbase.str();
   o << "  if (tid == 0u) {\n";
   for (size_t gi = 0; gi < NG; ++gi) o << "    stg[" << gi << "] = R" << gi << ";\n";
   for (size_t j = 0; j < nested.size(); ++j) o << "    stg[" << NG + j << "] = Q" << nested[j] << ";\n";
+  for (size_t gi = 0; gi < NG; ++gi) o << "    stg[" << NR + gi << "] = b" << group_scope(gi) << " & 31u;\n";
   o << "  }\n";
   for (size_t gi = 0; gi < NG; ++gi) {
-    const uint32_t s = group_scope(gi), AW = group_words(gi);
-    o << "  {   // exports of scope " << s << " (row loop " << gi << ")\n    const uint32_t* __restrict__ src = xs + X" << gi << " + (size_t)b" << s << " * " << AW << "u;\n"
-      << "    for (uint32_t i = tid; i < c" << s << " * " << AW << "u; i += nthr) GK_SPEC_CP4(stg + R" << gi << " + i, src + i);\n  }\n";
+    const uint32_t s = group_scope(gi), P = group_planes(gi);
+    if (!P) continue;
+    o << "  {   // planes of scope " << s << " (row loop " << gi << "): blocks b / 32 to ceil((b + c) / 32), the last for the windows' high words\n"
+      << "    const uint4* __restrict__ src = reinterpret_cast<const uint4*>(xs + X" << gi << " + (size_t)(b" << s << " >> 5) * " << P << "u);\n"
+      << "    uint4* dst = reinterpret_cast<uint4*>(stg + R" << gi << ");\n"
+      << "    const uint32_t n = (((b" << s << " & 31u) + c" << s << " + 31u) / 32u + 1u) * " << P / 4 << "u;\n"
+      << "    for (uint32_t i = tid; i < n; i += nthr) GK_SPEC_CP16(dst + i, src + i);\n  }\n";
   }
   // the offsets of sibling scopes are read at the same parent rows: one item stages all of a parent's children (independent loads)
   std::map<uint32_t, std::vector<uint32_t>> children;
@@ -1105,36 +1158,36 @@ struct uint4 { uint32_t x, y, z, w; };
     scope_extent(s, [&](const std::string& row) { return "q" + std::to_string(s) + "[" + row + "]"; });
     o << "  const uint32_t f" << s << " = n" << s << " >= 32u ? 0xffffffffu : ((1u << n" << s << ") - 1u);\n  (void)hi" << s << "; (void)f" << s << ";\n";
   }
-  std::vector<uint8_t> group_done(groups.size(), 0), any_done(g.nvar, 0);
-  auto emit_group = [&](size_t gi) {
-    if (group_done[gi]) return;
-    group_done[gi] = 1;
-    const std::vector<uint32_t>& ex = exports[gi];
-    const uint32_t s = group_scope(gi), AW = group_words(gi), AN = (nany[gi] + 31u) / 32u;
-    o << "  // ---- exports of scope " << s << " (row loop " << gi << "): the bits gk_spec_stage() left for the object's rows; x" << gi << "_<w> = the OR of the rows' words\n";
-    o << "  const uint32_t* __restrict__ a" << gi << " = stg + stg[" << gi << "];\n";
-    if (AN || ex.size() > nany[gi]) o << "  uint32_t";
-    for (uint32_t w = 0; w < AN; ++w) o << (w ? ", x" : " x") << gi << "_" << w << " = 0u";
-    for (size_t k = nany[gi]; k < ex.size(); ++k) o << (k || AN ? ", v" : " v") << ex[k] << " = 0u";
-    o << ";\n";
-    if (s == 0) o << "  {\n    const uint32_t row = o;\n    const uint32_t bit = 1u;\n";
-    else o << "  _Pragma(\"unroll 1\") for (uint32_t j = 0; j < n" << s << "; ++j) {\n    const uint32_t row = lo" << s << " + j;\n    const uint32_t bit = 1u << j;\n";
-    o << "    (void)bit;\n    const uint32_t";
-    for (uint32_t w = 0; w < AW; ++w) o << (w ? ", w" : " w") << w << " = a" << gi << "[" << AW << "u * row + " << w << "u]";
-    o << ";\n";
-    for (uint32_t w = 0; w < AN; ++w) o << "    x" << gi << "_" << w << " |= w" << w << ";\n";
-    for (size_t k = nany[gi]; k < ex.size(); ++k) o << "    if (w" << k / 32 << " & " << hx(1u << (k % 32)) << ") v" << ex[k] << " |= bit;\n";
-    o << "  }\n";
+  // the object's rows of scope s start at bit e<g> of row loop g's staged planes: plane k's 32-bit window there, bit j = row j of the
+  // object, is the mask of export k (masked to the object's rows, f<s>); an export only object-level EXISTS read is that mask != 0.
+  // On the object's own row (f0 = 1) the window is one bit of the low word.  Each window is taken where the walk first reads it.
+  std::vector<uint8_t> group_done(groups.size(), 0), window_done(g.nvar, 0);
+  std::vector<int> plane_of(g.nvar, -1);
+  for (size_t gi = 0; gi < NG; ++gi)
+    for (size_t k = 0; k < exports[gi].size(); ++k) plane_of[exports[gi][k]] = (int)k;
+  auto emit_window = [&](size_t gi, uint32_t v) {
+    const std::string G = std::to_string(gi), S = std::to_string(group_scope(gi));
+    const uint32_t P = group_planes(gi), k = (uint32_t)plane_of[v];
+    if (!group_done[gi]) {
+      group_done[gi] = 1;
+      o << "  // ---- exports of scope " << S << " (row loop " << gi << "): windows of the planes gk_spec_stage() left, from the object's first row\n";
+      o << "  const uint32_t e" << G << " = lo" << S << " + stg[" << NR + gi << "], sh" << G << " = e" << G << " & 31u;\n";
+      o << "  const uint32_t* __restrict__ pl" << G << " = stg + stg[" << gi << "] + (e" << G << " >> 5) * " << P << "u;\n";
+    }
+    if (group_scope(gi) == 0) {
+      o << "  const uint32_t v" << v << " = (pl" << G << "[" << k << "] >> sh" << G << ") & 1u;\n";
+    } else {
+      const std::string win = "GK_SPEC_FUNNEL(pl" + G + "[" + std::to_string(k) + "], pl" + G + "[" + std::to_string(P + k) + "], sh" + G + ") & f" + S;
+      o << "  const uint32_t v" << v << " = " << (form[v] == kAny ? "(" + win + ") != 0u ? 1u : 0u" : win) << ";\n";
+    }
   };
   // ---- everything else depth-first from the results: a node right after what it reads.  The gates phase 1 evaluated are not nodes
   // here: the walk ends at the exports.
   std::function<void(uint32_t)> emit_var = [&](uint32_t v) {
     if (local[v] >= 0) {
-      const size_t gi = (size_t)group_ix.at((uint32_t)local[v]);
-      emit_group(gi);
-      if (form[v] == kAny && !any_done[v]) {   // (0 or 1: the object-level EXISTS that reads it tests `!= 0`)
-        any_done[v] = 1;
-        o << "  const uint32_t v" << v << " = (x" << gi << "_" << bit_of[v] / 32 << " >> " << bit_of[v] % 32 << ") & 1u;\n";
+      if (!window_done[v]) {
+        window_done[v] = 1;
+        emit_window((size_t)group_ix.at((uint32_t)local[v]), v);
       }
       return;
     }

@@ -4,9 +4,9 @@
 // op a work item some warp decodes, ~400 warp-instructions per object at the benchmark's 50 constraints.  The netlist is known when
 // the constraint set is compiled, so the engine also writes it out as straight-line code, constants as immediates, in two phases per
 // tile.  Phase 1, one thread per ROW: the row's atoms and every gate that reads that row alone, of which only the bits something
-// else reads (exports) are stored in shared memory.  Phase 2, one thread per OBJECT: every remaining node a 32-bit mask register
-// (bit j = row j of THIS object in the node's scope), an export that only object-level EXISTS read one bit of the OR of the rows'
-// words, EXISTS a `!= 0`, the object-major bitmap words assembled in registers without a transpose.  NVRTC compiles that text for
+// else reads (exports) are stored, as bit planes of 32-row blocks.  Phase 2, one thread per OBJECT: every remaining node a 32-bit mask
+// register (bit j = row j of THIS object in the node's scope), an export one 32-bit window of its plane from the object's first row,
+// EXISTS a `!= 0`, the object-major bitmap words assembled in registers without a transpose.  NVRTC compiles that text for
 // sm_90a when the first large batch is evaluated (kernels.cu).  Objects with more than 32 rows in some scope do not fit the mask registers: they are
 // handed to the interpreter one by one, or with their whole tile when a tile holds more than GK_HANDOVER_MAX (GkKParams::units):
 // gk_spec_plan_kernel lists them from the CSR offsets before the rows are evaluated, and the interpreter runs beside the two kernels.
@@ -25,9 +25,11 @@ struct SpecSource {
   size_t smem = 0;        // fixed dynamic shared memory of a launch (column / scope tables, enforcement-point mask, totals)
   size_t n_fast = 0, n_generic = 0;   // atoms emitted as immediates / as calls of the generic gk_atom()
   // the per-tile staging area behind the fixed part: `hdr` words, then one region per entry of `stage` (the first `ngroups` are the
-  // row loops' exports, in row-loop order; the rest the nested scopes' offsets)
+  // row loops' export planes, in row-loop order; the rest the nested scopes' offsets)
   struct StageRegion {
-    uint32_t scope, per_row, extra;   // words = (rows of `scope` in the tile) * per_row + extra
+    // a row loop: `planes` export planes (its exports rounded up to 4), one word per plane per block of 32 rows of `scope`; a
+    // nested scope's offsets: one word per row of `scope` (its parent) + 1 (planes = 0)
+    uint32_t scope, planes;
   };
   std::vector<StageRegion> stage;
   uint32_t stage_hdr = 0;
@@ -48,16 +50,21 @@ struct SpecSource {
     }
     return t;
   }
-  // bytes of the staging area for a batch whose largest tile has cap[s] rows in scope s
+  // bytes of the staging area for a batch whose largest tile has cap[s] rows in scope s: a tile's rows of a scope start anywhere in
+  // a block of 32, so they span at most ceil(cap / 32) + 1 blocks, and the region holds one more (gk_spec_stage)
   size_t stage_bytes(const std::vector<uint32_t>& cap) const {
     size_t w = stage_hdr;
-    for (const StageRegion& r : stage) w += (size_t)(r.scope < cap.size() ? cap[r.scope] : 0u) * r.per_row + r.extra;
+    for (size_t i = 0; i < stage.size(); ++i) {
+      const size_t rows = stage[i].scope < cap.size() ? cap[stage[i].scope] : 0u;
+      w += i < ngroups ? ((rows + 31) / 32 + 2) * stage[i].planes : rows + 1;
+    }
     return w * 4;
   }
-  // bytes of the export arrays (gk_spec_rows_kernel -> gk_spec_kernel) of a batch with rows[s] rows in scope s (rows[0] = objects)
+  // bytes of the export planes (gk_spec_rows_kernel -> gk_spec_kernel) of a batch with rows[s] rows in scope s (rows[0] = objects):
+  // per row loop, `planes` words per block of 32 rows and one guard block (a window's high word past the last block)
   size_t export_bytes(const std::vector<uint32_t>& rows) const {
     size_t w = 0;
-    for (uint32_t g = 0; g < ngroups; ++g) w += (size_t)(stage[g].scope < rows.size() ? rows[stage[g].scope] : 0u) * stage[g].per_row;
+    for (uint32_t g = 0; g < ngroups; ++g) w += (((stage[g].scope < rows.size() ? rows[stage[g].scope] : 0u) + (size_t)31) / 32 + 1) * stage[g].planes;
     return w * 4;
   }
   // blocks of gk_spec_rows_kernel over such a batch at `threads` per block
