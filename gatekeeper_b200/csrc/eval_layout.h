@@ -58,6 +58,53 @@ inline uint64_t gk_slot_layout(const std::vector<uint8_t>& slot_level, const std
   return words;
 }
 
+// The type words of a batch (program.h): which scopes have them, which column is which nibble, and where each scope's words lie
+// in the batch's one type-word allocation.  Computed from the column table alone, so the backend's allocation and pack pass, the
+// code generator and the generated text's host build all take it from here.
+struct GkTwLayout {
+  std::vector<uint32_t> words;                // per scope: W_s, words per row (0: no type words)
+  std::vector<std::vector<uint32_t>> vtcols;  // per scope with words: its VT columns in nibble order (column-index order)
+  std::vector<uint32_t> nibble;               // per column: its nibble in its scope's row, or GK_NONE (no VT, or no words in the scope)
+  bool operator==(const GkTwLayout& o) const { return words == o.words && vtcols == o.vtcols; }
+  // the allocation of a batch with rows[s] rows in scope s: the per-scope pointer table (nscopes pointers), then each scope's
+  // words, every region 16-byte aligned; `at` (if not null) gets every scope's byte offset (0: no words)
+  size_t bytes(const std::vector<uint32_t>& rows, std::vector<size_t>* at) const {
+    auto r16 = [](size_t b) { return (b + 15) / 16 * 16; };
+    size_t off = r16(words.size() * 8);
+    if (at) at->assign(words.size(), 0);
+    for (size_t s = 0; s < words.size(); ++s) {
+      if (!words[s]) continue;
+      if (at) (*at)[s] = off;
+      off += r16((s < rows.size() ? rows[s] : 0u) * (size_t)words[s] * 4);
+    }
+    return off;
+  }
+  bool any() const {
+    for (uint32_t w : words)
+      if (w) return true;
+    return false;
+  }
+};
+// cols: the batch's column table, anything with `scope` and `enc` (GkColumn, the schema's column definitions)
+template <class Col>
+inline GkTwLayout gk_tw_layout(const std::vector<Col>& cols, size_t nscopes) {
+  GkTwLayout L;
+  L.words.assign(nscopes, 0);
+  L.vtcols.assign(nscopes, {});
+  L.nibble.assign(cols.size(), GK_NONE);
+  for (size_t ci = 0; ci < cols.size(); ++ci)
+    if ((cols[ci].enc & GK_ENC_VT) && (size_t)cols[ci].scope < nscopes) L.vtcols[(size_t)cols[ci].scope].push_back((uint32_t)ci);
+  for (size_t s = 0; s < nscopes; ++s) {
+    L.words[s] = gk_tw_words((uint32_t)L.vtcols[s].size());
+    if (!L.words[s]) {
+      L.vtcols[s].clear();
+      continue;
+    }
+    for (size_t k = 0; k < L.vtcols[s].size(); ++k) L.nibble[L.vtcols[s][k]] = (uint32_t)k;
+  }
+  return L;
+}
+
 // What one netlist needs in shared memory besides the tile: the table counts gk_eval_layout takes and the scope of every slot.
 struct GkNetSize {
   uint32_t C, NS, NP, nops, nitems, nmatch, ncols, npool, ncbytes;

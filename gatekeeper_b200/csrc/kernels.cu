@@ -75,6 +75,11 @@ struct DevBatch {
   unsigned long long* gvk = nullptr;   // [n] hash of (apiVersion, kind) per object, 0 for a skipped one (audit_candidates)
   std::vector<uint32_t> cap;  // rows of the largest tile per scope (sizes the slot area of any netlist over this batch)
   std::vector<uint32_t> rows; // rows per scope in the batch, rows[0] = objects (sizes the generated kernel's export arrays)
+  // the type words (program.h): pointer table and every packed scope's words, laid out by `tw` (pack_type_words); a fork's are its
+  // batch's
+  uint8_t* d_tw = nullptr;
+  size_t tw_bytes = 0;
+  GkTwLayout tw;
   bool fork = false;          // a view made by fork_batch: arena and tiling belong to the batch it was forked from
   // a resultant batch of an expanded batch (set_parents): its parents as a CSR, and the totals its own evaluations write
   uint32_t* fold_par = nullptr;
@@ -231,6 +236,11 @@ __global__ void gk_sel_emit_kernel(const uint32_t* viol, const uint32_t* rank, c
     }
     cand[i] = out;
   }
+}
+
+// the type words of one scope (program.h), one thread per row
+__global__ void gk_tw_pack_kernel(const GkColumn* cols, const uint32_t* vtcols, uint32_t nvt, uint32_t W, uint32_t rows, uint32_t* dst) {
+  for (size_t row = (size_t)blockIdx.x * blockDim.x + threadIdx.x; row < rows; row += (size_t)gridDim.x * blockDim.x) gk_tw_pack_row(cols, vtcols, nvt, W, row, dst);
 }
 
 // ---- expanded batches (Backend::select_generators, eval_expanded, fold_into)
@@ -472,6 +482,7 @@ class CudaBackend : public Backend {
       CK(cudaMemcpyAsync(db->d_tile_lo, tile_lo.data(), tile_lo.size() * 4, cudaMemcpyHostToDevice, stream_));
       if (hb.n) CK(cudaMemcpyAsync(db->gvk, hb.gvk.data(), (size_t)hb.n * 8, cudaMemcpyHostToDevice, stream_));
       CK(cudaEventRecord(b, stream_));
+      pack_type_words(db, c);
       CK(cudaStreamSynchronize(stream_));
     }
     float ms = 0;
@@ -492,6 +503,46 @@ class CudaBackend : public Backend {
                         (uint32_t)k->items.size(), (uint32_t)k->match.size(), (uint32_t)k->schema.cols.size(), (uint32_t)k->pool.size(),
                         (uint32_t)k->cbytes.size(), k->slot_level});
     return nets;
+  }
+
+  // The type words of a batch whose columns are resident, or are being copied there on stream_ (program.h): derived on the device from
+  // the VT byte columns, which stay (the interpreter reads them), one pass per scope that has them.  upload() and extract(), every
+  // path by which a batch's columns become resident, end here; the caller synchronises stream_ before the batch is evaluated.
+  void pack_type_words(DevBatch* db, const Compiled& c) {
+    const size_t NS = c.schema.scopes.size();
+    db->tw = gk_tw_layout(c.schema.cols, NS);
+    if (!db->tw.any()) return;
+    std::vector<size_t> at;
+    db->tw_bytes = db->tw.bytes(db->rows, &at);
+    std::vector<uint32_t> vc;   // every scope's VT columns, back to back
+    std::vector<size_t> vc_at(NS, 0);
+    for (size_t s = 0; s < NS; ++s) {
+      vc_at[s] = vc.size();
+      vc.insert(vc.end(), db->tw.vtcols[s].begin(), db->tw.vtcols[s].end());
+    }
+    // the layout's allocation (pointer table, words), then the column lists the pack pass reads
+    dmalloc(&db->d_tw, db->tw_bytes + vc.size() * 4);
+    std::vector<uint64_t> ptr(NS, 0);
+    for (size_t s = 0; s < NS; ++s)
+      if (db->tw.words[s]) ptr[s] = reinterpret_cast<uint64_t>(db->d_tw + at[s]);
+    push_small(db->d_tw, ptr.data(), NS * 8);
+    uint32_t* d_vc = reinterpret_cast<uint32_t*>(db->d_tw + db->tw_bytes);
+    push_small(d_vc, vc.data(), vc.size() * 4);
+    for (size_t s = 0; s < NS; ++s) {
+      const uint32_t rows = s < db->rows.size() ? db->rows[s] : 0u;
+      if (!db->tw.words[s] || !rows) continue;
+      gk_tw_pack_kernel<<<std::min<uint32_t>((rows + 255u) / 256u, (uint32_t)sms_ * 16u), 256, 0, stream_>>>(
+          db->hdr.cols, d_vc + vc_at[s], (uint32_t)db->tw.vtcols[s].size(), db->tw.words[s], rows, reinterpret_cast<uint32_t*>(db->d_tw + at[s]));
+      CK(cudaGetLastError());
+      ++launches_;
+    }
+    db->hdr.tw = reinterpret_cast<const uint32_t* const*>(db->d_tw);
+    if (getenv("GK_TRACE_LAUNCH")) {
+      std::string line = "[launch] type words:";
+      for (size_t s = 0; s < NS; ++s)
+        if (db->tw.words[s]) line += " scope " + std::to_string(s) + ": " + std::to_string(db->tw.vtcols[s].size()) + " vt columns in " + std::to_string(db->tw.words[s]) + " words;";
+      fprintf(stderr, "%s %zu bytes for %u objects\n", line.c_str(), db->tw_bytes, db->n);
+    }
   }
 
   // slot area of a tile from the per-scope tile capacities; the netlist with slot ids resolved to word offsets; output planes
@@ -611,6 +662,7 @@ class CudaBackend : public Backend {
     dfree(db->d_ops);
     dfree(db->d_pool);
     dfree(db->d_outs);
+    dfree(db->d_tw);
     delete db;
   }
 
@@ -659,6 +711,8 @@ class CudaBackend : public Backend {
       // The generated kernel stages the largest tile's rows in shared memory: one bit per row per export plane of a scope that has
       // atoms, where the interpreter holds one bit per row per live slot.  A scope with many rows in a tile can therefore need more
       // than the device allows while the interpreter fits: that batch is interpreted.
+      // (the rows read the batch's type words as the text lays them out: both come from gk_tw_layout over the same columns)
+      if (!(spec_cur_->src.tw == db->tw)) throw BackendError{"batch type words are laid out for another column table"};
       spec_smem_ = spec_cur_->src.smem + spec_cur_->src.stage_bytes(db->cap);
       spec_next_ = spec_smem_ <= spec_cur_->max_smem;
       spec_per_sm_ = 0;   // resident CTAs per SM: the persistent grid of fire()
@@ -1572,6 +1626,7 @@ class CudaBackend : public Backend {
     db->tile = tile;
     db->ntiles = ntiles;
     db->gvk_uniform = mm[1] == 0 || mm[0] == mm[1];
+    pack_type_words(db, c);
     finish_batch(db, c, cap);
     if (st) {
       float ms = 0;
@@ -1617,6 +1672,8 @@ class CudaBackend : public Backend {
     f->gvk_uniform = db->gvk_uniform;
     f->gvk = db->gvk;
     f->rows = db->rows;
+    f->tw = db->tw;   // (f->hdr.tw: the batch's type words, which it keeps)
+    f->tw_bytes = db->tw_bytes;
     f->fork = true;
     f->prog_version = other.version;
     std::unique_ptr<DevBatch, std::function<void(DevBatch*)>> guard(f, [this](DevBatch* x) { release(x); });

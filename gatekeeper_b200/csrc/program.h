@@ -99,7 +99,29 @@ typedef struct {
   const GkColumn* cols;
   const GkScope* scopes;
   uint32_t ncols, nscopes;
+  // [nscopes] the type words of every scope (gk_tw_layout, eval_layout.h): tw[s][row * W_s + w], null for a scope without them.
+  // A derived copy of the VT columns, made where the batch becomes resident; only the generated kernel's rows read it.
+  const uint32_t* const* tw;
 } GkBatch;
+
+// ---- type words: the VT values of one row of a scope, 4 bits each (GK_VT_* < 16), 8 per 32-bit word.  A row's words are one
+// aligned load where its VT columns are one byte load each.  Nibble k of a row is the k-th VT column of the scope in column order;
+// its value is (tw[row * W + k / 8] >> 4 * (k % 8)) & 15.  gk_tw_layout (eval_layout.h) decides which scopes have them.
+#define GK_TW_MIN 4u   /* VT columns a scope needs for type words: below that its byte loads cost no more */
+// words per row of a scope with nvt VT columns: none below GK_TW_MIN, else ceil(nvt / 8) rounded up to 1, 2 or a multiple of 4,
+// so that a row is one 4- or 8-byte load or whole 16-byte loads
+GK_HD uint32_t gk_tw_words(uint32_t nvt) {
+  const uint32_t w = (nvt + 7u) / 8u;
+  return nvt < GK_TW_MIN ? 0u : w <= 2u ? w : (w + 3u) & ~3u;
+}
+// one row of one scope: its nvt VT columns (column indices in nibble order) into its W words
+GK_HD void gk_tw_pack_row(const GkColumn* cols, const uint32_t* vtcols, uint32_t nvt, uint32_t W, size_t row, uint32_t* dst) {
+  for (uint32_t w = 0; w < W; ++w) {
+    uint32_t x = 0u;
+    for (uint32_t k = 8u * w; k < nvt && k < 8u * w + 8u; ++k) x |= ((uint32_t)GK_LD(cols[vtcols[k]].vt + row) & 15u) << (4u * (k & 7u));
+    dst[(size_t)row * W + w] = x;
+  }
+}
 
 // ---- match block
 enum { GK_M_HAS_MATCH = 1, GK_M_SCOPE_CLUSTER = 2, GK_M_SCOPE_NAMESPACED = 4, GK_M_HAS_LSEL = 8, GK_M_HAS_NSSEL = 16,

@@ -213,6 +213,22 @@ static uint32_t gk_spec_host_plan(const GkBatch& B, uint32_t tile, std::vector<u
 #define GK_SPEC_HOST_TILE 96u
 #endif
 extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint32_t* ew) {
+  // the batch's type words, packed again at its first object (the backend packs them where the batch becomes resident)
+  struct Types {
+    const void* flags = nullptr;
+    uint32_t n = 0;
+    std::vector<std::vector<uint32_t>> words;
+    std::vector<const uint32_t*> ptrs;
+  };
+  static thread_local Types ty;
+  if (obj == 0u || ty.flags != (const void*)p->batch.flags || ty.n != p->batch.n) {
+    gk_spec_host_types(p->batch, ty.words, ty.ptrs);
+    ty.flags = p->batch.flags;
+    ty.n = p->batch.n;
+  }
+  GkKParams pt = *p;
+  pt.batch.tw = ty.ptrs.data();
+  p = &pt;
   uint32_t actw[GK_SPEC_W];
   for (uint32_t w = 0; w < GK_SPEC_W; ++w) vw[w] = ew[w] = actw[w] = 0u;
   for (uint32_t c = 0; c < GK_SPEC_C; ++c)
@@ -711,6 +727,7 @@ SpecSource spec_codegen(const Compiled& c) {
   const size_t NS = c.schema.scopes.size();
   Gen g(c);
   g.use_scope(0);
+  out.tw = gk_tw_layout(c.schema.cols, NS);
   for (const GkOp& op : c.ops) {
     const uint32_t kind = op.w0 & 0xffu;
     if (kind == GK_N_END) break;
@@ -742,6 +759,7 @@ SpecSource spec_codegen(const Compiled& c) {
       out.errlist[3 * sl_ + 2] = (code);                             \
     }                                                                \
   }
+struct uint2 { uint32_t x, y; };
 struct uint4 { uint32_t x, y, z, w; };
 #define GK_SPEC_CP16(d, s) (*(d) = *(s))
 #define GK_SPEC_CP_WAIT()
@@ -1003,10 +1021,38 @@ __device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
     o << "\n// atoms, row-local gates" << (s == 0 && !match_at[0].empty() ? ", spec.match blocks" : "") << " and exports of one row of scope " << s << " (row loop " << gi << ")\n";
     o << "GK_SPEC_FN void gk_spec_row_" << gi << "(const GkBatch& B, const GkColumn* cols, const uint32_t* __restrict__ pool, const uint8_t* __restrict__ cbytes, const GkOut& out,\n"
       << "                              const size_t row, uint32_t* __restrict__ a) {\n  (void)B; (void)cols; (void)pool; (void)cbytes; (void)out; (void)a;\n";
+    // the row's type words, when its scope has them (gk_tw_layout) and an atom reads a type: one aligned 4- or 8-byte load, or one
+    // 16-byte load per 4 words, and every tK a nibble of them instead of a byte load of its own
+    const uint32_t TW = s < out.tw.words.size() ? out.tw.words[s] : 0u;
+    auto packed = [&](uint32_t ci) { return TW && ci < out.tw.nibble.size() && out.tw.nibble[ci] != GK_NONE && (uint32_t)c.schema.cols[ci].scope == s; };
+    bool any_packed = false;
+    for (auto& kv : need) any_packed = any_packed || ((kv.second & GK_ENC_VT) && packed(kv.first));
+    if (any_packed) {
+      o << "  const uint32_t* __restrict__ tws = B.tw[" << s << "];\n";
+      if (TW == 1) {
+        o << "  const uint32_t tw0 = GK_SPEC_LD(tws + row);\n";
+      } else if (TW == 2) {
+        o << "  const uint2 twv = GK_SPEC_LD(reinterpret_cast<const uint2*>(tws) + row);\n  const uint32_t tw0 = twv.x, tw1 = twv.y;\n";
+      } else {
+        for (uint32_t j = 0; j < TW / 4; ++j) {
+          const std::string J = std::to_string(j), q = std::to_string(4 * j);
+          o << "  const uint4 twv" << J << " = GK_SPEC_LD(reinterpret_cast<const uint4*>(tws) + row * " << TW / 4 << "u + " << j << "u);\n";
+          o << "  const uint32_t tw" << q << " = twv" << J << ".x, tw" << 4 * j + 1 << " = twv" << J << ".y, tw" << 4 * j + 2 << " = twv" << J << ".z, tw" << 4 * j + 3 << " = twv"
+            << J << ".w;\n";
+        }
+      }
+      for (uint32_t w = 0; w < TW; ++w) o << (w ? " " : "  ") << "(void)tw" << w << ";";
+      o << "\n";
+    }
     for (auto& kv : need) {
       const uint32_t ci = kv.first, enc = kv.second;
       const std::string K = std::to_string(ci);
-      if (enc & GK_ENC_VT) o << "  const uint32_t t" << K << " = GK_SPEC_LD(cols[" << K << "].vt + row);\n";
+      if ((enc & GK_ENC_VT) && packed(ci)) {
+        const uint32_t k = out.tw.nibble[ci];
+        o << "  const uint32_t t" << K << " = (tw" << k / 8 << " >> " << 4 * (k % 8) << "u) & 15u;\n";
+      } else if (enc & GK_ENC_VT) {
+        o << "  const uint32_t t" << K << " = GK_SPEC_LD(cols[" << K << "].vt + row);\n";
+      }
       if (enc & GK_ENC_SID) o << "  const uint32_t i" << K << " = GK_SPEC_LD(cols[" << K << "].sid + row);\n";
       if (enc & GK_ENC_NUM) o << "  const long long n" << K << " = GK_SPEC_LD(reinterpret_cast<const long long*>(cols[" << K << "].num) + row);\n";
       if (enc & GK_ENC_HEAD)
@@ -1049,12 +1095,35 @@ __device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
   o << "}\n";
   o << "static size_t gk_spec_export_words(const GkBatch& B) {\n  const GkScope* scopes = B.scopes;\n" << xbase.str() << "  return X" << NG << ";\n}\n";
   // GK_SPEC_TRACE: "[spec planes] loop <g>: scope <s>, <exports> exports, <rows> rows; ...; <words> export words" (once per batch)
-  o << "#include <cstdio>\nstatic void gk_spec_trace_planes(const GkBatch& B) {\n  fprintf(stderr, \"[spec planes]\");\n";
+  o << "#include <cstdio>\n#include <vector>\nstatic void gk_spec_trace_planes(const GkBatch& B) {\n  fprintf(stderr, \"[spec planes]\");\n";
   for (size_t gi = 0; gi < NG; ++gi) {
     const uint32_t s = group_scope(gi);
     o << "  fprintf(stderr, \" loop " << gi << ": scope " << s << ", " << exports[gi].size() << " exports, %u rows;\", " << (s ? "B.scopes[" + std::to_string(s) + "].rows" : std::string("B.n")) << ");\n";
   }
-  o << "  fprintf(stderr, \" %zu export words\\n\", gk_spec_export_words(B));\n}\n";
+  o << "  fprintf(stderr, \" %zu export words\\n\", gk_spec_export_words(B));\n";
+  // "[spec types] scope <s>: <vt columns> vt columns in <W> words, <rows> rows; ...; <bytes> type-word bytes" (the scopes with type words)
+  o << "  size_t twb = 0;\n  fprintf(stderr, \"[spec types]\");\n";
+  for (size_t s = 0; s < NS; ++s) {
+    if (!out.tw.words[s]) continue;
+    const std::string R = s ? "B.scopes[" + std::to_string(s) + "].rows" : std::string("B.n");
+    o << "  fprintf(stderr, \" scope " << s << ": " << out.tw.vtcols[s].size() << " vt columns in " << out.tw.words[s] << " words, %u rows;\", " << R << ");\n  twb += (size_t)"
+      << R << " * " << out.tw.words[s] * 4 << "u;\n";
+  }
+  o << "  fprintf(stderr, \" %zu type-word bytes\\n\", twb);\n}\n";
+  // the type words of the whole batch, as the backend's pack pass makes them (gk_tw_pack_row over the same layout), into `words`;
+  // returns the per-scope pointer table for GkBatch::tw
+  o << "static const uint32_t* const* gk_spec_host_types(const GkBatch& B, std::vector<std::vector<uint32_t>>& words, std::vector<const uint32_t*>& ptrs) {\n"
+    << "  words.assign(" << NS << "u, std::vector<uint32_t>());\n  ptrs.assign(" << NS << "u, nullptr);\n";
+  for (size_t s = 0; s < NS; ++s) {
+    if (!out.tw.words[s]) continue;
+    const std::vector<uint32_t>& vc = out.tw.vtcols[s];
+    o << "  {\n    static const uint32_t vc[" << vc.size() << "] = {";
+    for (size_t k = 0; k < vc.size(); ++k) o << (k ? ", " : "") << vc[k] << "u";
+    o << "};\n    const uint32_t rows = " << (s ? "B.scopes[" + std::to_string(s) + "].rows" : std::string("B.n")) << ";\n    words[" << s << "].assign((size_t)rows * "
+      << out.tw.words[s] << "u + 1u, 0xdeadbeefu);\n    for (size_t row = 0; row < rows; ++row) gk_tw_pack_row(B.cols, vc, " << vc.size() << "u, " << out.tw.words[s]
+      << "u, row, words[" << s << "].data());\n    ptrs[" << s << "] = words[" << s << "].data();\n  }\n";
+  }
+  o << "  return ptrs.data();\n}\n";
   // (the rows of the tile [tlo, thi) only, and of those only their own bits of the plane words: a copy, or a window, that reads a row
   // outside them finds the caller's poison)
   o << "static void gk_spec_host_rows(const GkKParams* p, const uint32_t* tlo, const uint32_t* thi, uint32_t* xs) {\n  const GkBatch& B = p->batch;\n  const GkScope* scopes = B.scopes;\n"

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "engine.hpp"
+#include "eval_layout.h"
 
 namespace gk {
 
@@ -40,6 +41,9 @@ struct SpecSource {
     uint32_t scope, atoms, gates, any, mask, words;
   };
   std::vector<Fold> fold;
+  // the type words the rows read (gk_tw_layout of the constraint set's columns): a batch evaluated with this text must have them
+  // laid out alike
+  GkTwLayout tw;
   // "folded: scope S: A atoms + G gates -> X any + Y mask in W words; ..." (the first line of `src`, and the backend's trace)
   std::string fold_text() const {
     std::string t = "folded:";
