@@ -64,6 +64,7 @@ struct DevBatch {
   uint32_t* d_whole = nullptr;       // [ntiles + 1] the tiles handed over whole (GkKParams::whole), then the count of d_units
   uint64_t planned = 0;              // the constraint-set version whose hand-over plan d_units / d_whole hold (0: none yet)
   uint32_t nunits = 0;               // the plan's unit count
+  uint32_t multi = 0;                // of those, units of more than one object (a whole tile's wide objects)
   uint64_t handed = 0;               // the objects those units cover
   // the netlist with every slot id replaced by the slot's word offset in this batch's shared-memory slot area
   GkOp* d_ops = nullptr;
@@ -462,9 +463,7 @@ class CudaBackend : public Backend {
     if (hb.n) dmalloc(&db->gvk, (size_t)hb.n * 8);
     finish_batch(db, c, cap);
     const size_t tables_bytes = c.ops.size() * sizeof(GkOp) + c.pool.size() * 4 + c.outs.size() * sizeof(GkOutEnt);
-    cudaEvent_t a, b;
-    CK(cudaEventCreate(&a));
-    CK(cudaEventCreate(&b));
+    Event a, b;
     {
       std::lock_guard<std::mutex> l(mu_);
       // the arena image is assembled by all host threads directly in pinned memory (one copy of every byte), its
@@ -487,8 +486,6 @@ class CudaBackend : public Backend {
     }
     float ms = 0;
     cudaEventElapsedTime(&ms, a, b);
-    cudaEventDestroy(a);
-    cudaEventDestroy(b);
     if (h2d_ms) *h2d_ms = ms;
     if (h2d_bytes) *h2d_bytes = plan.total + tile_lo.size() * 4 + tables_bytes;
     return db;
@@ -645,6 +642,34 @@ class CudaBackend : public Backend {
   void dfree(void* p) {
     if (p) cudaFreeAsync(p, stream_);
   }
+  // stream-ordered scratch of one call: every take() is freed on stream_ when the call returns or throws
+  struct Temps {
+    CudaBackend* be;
+    std::vector<void*> held;
+    explicit Temps(CudaBackend* b) : be(b) {}
+    Temps(const Temps&) = delete;
+    Temps& operator=(const Temps&) = delete;
+    ~Temps() {
+      for (void* p : held) be->dfree(p);
+    }
+    template <class T = void>
+    T* take(size_t bytes) {
+      T* p = nullptr;
+      be->dmalloc(&p, bytes);
+      held.push_back(p);
+      return p;
+    }
+  };
+  // a timing event of one call, destroyed when the call returns or throws (those of a call are locals, so a failed create destroys
+  // the ones already made)
+  struct Event {
+    cudaEvent_t e = nullptr;
+    Event() { CK(cudaEventCreate(&e)); }
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    ~Event() { cudaEventDestroy(e); }
+    operator cudaEvent_t() const { return e; }
+  };
   void release(void* b) override {
     auto* db = static_cast<DevBatch*>(b);
     if (!db) return;
@@ -666,12 +691,46 @@ class CudaBackend : public Backend {
     delete db;
   }
 
-  // everything a launch needs besides the kernel itself (kept outside the timed region)
-  KParams prepare(DevBatch* db, const std::vector<uint32_t>& active, uint32_t* viol, uint32_t* err, unsigned long long* totals,
-                  unsigned long long* err_totals, cudaStream_t st, size_t* smem_out) {
+  // One evaluation as prepare() decides it and fire() carries it out: the interpreter's parameters and, when the kernel generated
+  // for the constraint set runs, that kernel and its sizes.
+  struct SpecEntry;
+  struct Launch {
+    KParams p;
+    size_t smem = 0;             // the interpreter's dynamic shared memory per CTA
+    cudaStream_t st = nullptr;
+    SpecEntry* spec = nullptr;   // the generated kernel, or null: the interpreter alone
+    uint32_t* x = nullptr;       // its export arrays
+    size_t spec_smem = 0;        // its dynamic shared memory per CTA
+    int spec_per_sm = 1;         // its resident CTAs per SM at that size
+    uint32_t rows_grid = 0;      // blocks of the rows kernel
+    uint32_t units = 0;          // units the interpreter evaluates beside it (the batch's hand-over plan)
+    uint32_t multi = 0;          // of those, units of more than one object
+    uint64_t handed = 0;         // the objects they cover
+  };
+
+  // the fused exchange's peer addressing, from the caller's DevOutPtrs into GkKParams or GkFoldArgs.  Called before anything is zeroed
+  // or launched (first in prepare(), and in fold_into() before the resultants' evaluation): bad addressing leaves the caller's buffers
+  // untouched.
+  template <class A>
+  static void set_peers(A& a, const DevOutPtrs& dst) {
+    if (dst.npeers > GK_MAX_PEERS || (dst.npeers && dst.rank >= dst.npeers)) throw BackendError{"bad peer addressing for the fused exchange"};
+    a.npeers = dst.npeers;
+    a.tot_stride = dst.tot_stride;
+    for (uint32_t q = 0; q < GK_MAX_PEERS; ++q) {
+      a.peer_viol[q] = q < dst.npeers ? reinterpret_cast<uint32_t*>(dst.peer_viol[q]) : nullptr;
+      a.peer_tot[q] = q < dst.npeers ? reinterpret_cast<unsigned long long*>(dst.peer_tot[q]) : nullptr;
+    }
+  }
+
+  // everything a launch needs besides the kernels themselves (kept outside the timed region); `peers`: eval_into()'s fused exchange
+  Launch prepare(DevBatch* db, const std::vector<uint32_t>& active, uint32_t* viol, uint32_t* err, unsigned long long* totals,
+                 unsigned long long* err_totals, cudaStream_t st, const DevOutPtrs& peers = DevOutPtrs{}) {
     const uint32_t C = prog_.nconstraints;
     if (db->prog_version != version_) throw BackendError{"batch was uploaded for another constraint set"};
-    KParams p;
+    Launch l;
+    l.st = st;
+    KParams& p = l.p;
+    set_peers(p, peers);
     p.batch = db->hdr;
     p.batch.dict_off = d_dict_off_;
     p.batch.dict_bytes = d_dict_bytes_;
@@ -693,58 +752,55 @@ class CudaBackend : public Backend {
     p.ntiles = db->ntiles;
     p.tile = db->tile;
     p.slot_words = db->slot_words;
-    p.npeers = 0;
-    p.tot_stride = 0;
     p.done_ctr = reinterpret_cast<uint32_t*>(d_scalars_) + 4;   // zeroed with the error counter before every launch
     p.done_target = 0;   // (set by fire())
-    for (int q = 0; q < GK_MAX_PEERS; ++q) {
-      p.peer_viol[q] = nullptr;
-      p.peer_tot[q] = nullptr;
-    }
     p.timing = nullptr;
     p.units = db->d_units;
     p.whole = db->d_whole;
     p.unit_count = db->d_whole + db->ntiles;
     p.list_mode = 0;
-    spec_next_ = spec_ready(db->n);   // (an NVRTC run the first time: here, outside the timed region)
-    if (spec_next_) {
+    if (spec_ready(db->n)) {   // (an NVRTC run the first time: here, outside the timed region)
+      SpecEntry& se = *spec_cur_;
       // The generated kernel stages the largest tile's rows in shared memory: one bit per row per export plane of a scope that has
       // atoms, where the interpreter holds one bit per row per live slot.  A scope with many rows in a tile can therefore need more
       // than the device allows while the interpreter fits: that batch is interpreted.
       // (the rows read the batch's type words as the text lays them out: both come from gk_tw_layout over the same columns)
-      if (!(spec_cur_->src.tw == db->tw)) throw BackendError{"batch type words are laid out for another column table"};
-      spec_smem_ = spec_cur_->src.smem + spec_cur_->src.stage_bytes(db->cap);
-      spec_next_ = spec_smem_ <= spec_cur_->max_smem;
-      spec_per_sm_ = 0;   // resident CTAs per SM: the persistent grid of fire()
-      if (spec_next_ &&
-          cudaOccupancyMaxActiveBlocksPerMultiprocessor(&spec_per_sm_, reinterpret_cast<const void*>(spec_cur_->kern), spec_cur_->threads, spec_smem_) != cudaSuccess) {
+      if (!(se.src.tw == db->tw)) throw BackendError{"batch type words are laid out for another column table"};
+      l.spec_smem = se.src.smem + se.src.stage_bytes(db->cap);
+      bool run = l.spec_smem <= se.max_smem;
+      l.spec_per_sm = 0;   // resident CTAs per SM: the persistent grid of fire()
+      if (run && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&l.spec_per_sm, reinterpret_cast<const void*>(se.kern), se.threads, l.spec_smem) != cudaSuccess) {
         cudaGetLastError();
-        spec_per_sm_ = spec_minb_;
+        l.spec_per_sm = spec_minb_;
       }
-      spec_per_sm_ = std::max(1, spec_per_sm_);
+      l.spec_per_sm = std::max(1, l.spec_per_sm);
       // The hand-over plan depends on the batch's CSR offsets, which never change, and on the generated text: made by the first
-      // evaluation of the batch with this constraint set, here, and kept, with its unit count and the objects they cover on the host.
+      // evaluation of the batch with this constraint set, here, and kept, with its unit counts and the objects they cover on the host.
       // (It reads every offset array the netlist uses: at config 2 about as long as the interpreter's units take, so planning on
       // every evaluation would give back most of the overlap.)
-      if (spec_next_ && db->planned != spec_cur_->version && p.ntiles) {
+      if (run && db->planned != se.version && p.ntiles) {
         CK(cudaMemsetAsync(p.unit_count, 0, 4, st));
         void* args[] = {&p};
-        CK(cudaLaunchKernel(reinterpret_cast<const void*>(spec_cur_->plan_kern), dim3(p.ntiles), dim3(256), args, 0, st));
+        CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.plan_kern), dim3(p.ntiles), dim3(256), args, 0, st));
         ++launches_;
         CK(cudaMemcpyAsync(&db->nunits, p.unit_count, 4, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         std::vector<uint32_t> u((size_t)db->nunits * 2);
         if (db->nunits) CK(cudaMemcpy(u.data(), p.units, u.size() * 4, cudaMemcpyDeviceToHost));
+        db->multi = 0;
         db->handed = 0;
-        for (uint32_t i = 0; i < db->nunits; ++i) db->handed += u[2 * i + 1];
-        db->planned = spec_cur_->version;
+        for (uint32_t i = 0; i < db->nunits; ++i) {
+          db->multi += u[2 * i + 1] > 1u;
+          db->handed += u[2 * i + 1];
+        }
+        db->planned = se.version;
       }
       // A batch the plan hands over whole (every tile has more wide objects than GK_HANDOVER_MAX) is the interpreter's alone: the
       // rows and tile kernels would evaluate every row for nothing.
-      if (spec_next_ && p.ntiles && db->handed >= db->n) spec_next_ = false;
+      if (run && p.ntiles && db->handed >= db->n) run = false;
       // the export planes: scratch rewritten by every evaluation, grown (never shrunk) outside the timed region
-      const size_t xb = spec_cur_->src.export_bytes(db->rows);
-      if (spec_next_ && xb > spec_x_bytes_) {
+      const size_t xb = se.src.export_bytes(db->rows);
+      if (run && xb > spec_x_bytes_) {
         if (d_spec_x_) CK(cudaFree(d_spec_x_));
         d_spec_x_ = nullptr;
         spec_x_bytes_ = 0;
@@ -752,8 +808,14 @@ class CudaBackend : public Backend {
         spec_x_bytes_ = xb;
         if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[spec] export arrays: %zu bytes for %u objects\n", xb, db->n);
       }
-      spec_rows_grid_ = spec_cur_->src.rows_blocks(db->rows, (uint32_t)spec_cur_->rows_threads);
-      spec_units_ = db->nunits;
+      if (run) {
+        l.spec = &se;
+        l.x = d_spec_x_;
+        l.rows_grid = se.src.rows_blocks(db->rows, (uint32_t)se.rows_threads);
+        l.units = db->nunits;
+        l.multi = db->multi;
+        l.handed = db->handed;
+      }
     }
 #ifdef GK_PHASE_TIMING
     if (!d_timing_) CK(cudaMalloc(&d_timing_, (kMaxPhases + 2 + 16) * 16));
@@ -772,16 +834,18 @@ class CudaBackend : public Backend {
     if (C) CK(cudaMemsetAsync(err_totals, 0, (size_t)C * sizeof(unsigned long long), st));
     CK(cudaMemsetAsync(d_scalars_, 0, 64, st));
     // the kernel carves its shared memory with the same call on the same parameters
-    const size_t smem = gk_eval_layout(p.prog.nconstraints, p.batch.nscopes, p.prog.nphases, p.slot_words, p.prog.nops, p.prog.nitems, p.prog.nmatch,
-                                       p.batch.ncols, p.prog.npool, p.prog.ncbytes).total;
-    if (smem > max_smem_)
-      throw BackendError{"constraint set needs " + std::to_string(smem) + " bytes of shared memory per CTA (limit " + std::to_string(max_smem_) +
+    l.smem = gk_eval_layout(p.prog.nconstraints, p.batch.nscopes, p.prog.nphases, p.slot_words, p.prog.nops, p.prog.nitems, p.prog.nmatch,
+                            p.batch.ncols, p.prog.npool, p.prog.ncbytes).total;
+    if (l.smem > max_smem_)
+      throw BackendError{"constraint set needs " + std::to_string(l.smem) + " bytes of shared memory per CTA (limit " + std::to_string(max_smem_) +
                          "): too many live netlist columns for one launch"};
-    *smem_out = smem;
-    return p;
+    return l;
   }
 
-  void fire(KParams p, size_t smem, cudaStream_t st) {
+  void fire(Launch l) {
+    KParams& p = l.p;
+    const size_t smem = l.smem;
+    cudaStream_t st = l.st;
     if (p.ntiles == 0) return;
     // persistent CTAs: as many as fit per SM (shared-memory bound), each walks tiles with a grid stride
     int per_sm = 1;   // resident CTAs per SM for this launch configuration (registers and shared memory)
@@ -790,7 +854,7 @@ class CudaBackend : public Backend {
     if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[launch] %d CTAs/SM x %d threads, %zu B smem/CTA, %u tiles of %u objects\n", per_sm, kThreads, smem, p.ntiles, p.tile);
     uint32_t grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * per_sm)));
     last_kernel_ = "gk_eval_kernel";
-    if (!spec_next_) {
+    if (!l.spec) {
       p.done_target = grid;
       gk_eval_kernel<<<grid, kThreads, smem, st>>>(p);
       CK(cudaGetLastError());
@@ -805,14 +869,13 @@ class CudaBackend : public Backend {
     // kernel's pending blocks.  Neither grid waits for the other on the device: the two write disjoint words, add into the same
     // totals, and in the fused exchange the last CTA of either publishes (done_target).  A batch without units launches no
     // interpreter at all.
-    SpecEntry& se = *spec_cur_;
-    uint32_t* xs = d_spec_x_;
-    const uint32_t spec_grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * spec_per_sm_)));
+    SpecEntry& se = *l.spec;
+    const uint32_t spec_grid = std::max(1u, std::min<uint32_t>(p.ntiles, (uint32_t)(sms_ * l.spec_per_sm)));
     // the interpreter's persistent grid, each CTA striding over the list
     grid = std::max(1u, std::min<uint32_t>(p.batch.n, (uint32_t)(sms_ * per_sm)));
     p.list_mode = 1;
-    p.done_target = spec_grid + (spec_units_ ? grid : 0u);
-    if (spec_units_) {
+    p.done_target = spec_grid + (l.units ? grid : 0u);
+    if (l.units) {
       CK(cudaEventRecord(ev_fork_, st));
       CK(cudaStreamWaitEvent(side_stream_, ev_fork_, 0));
       gk_eval_kernel<<<grid, kThreads, smem, side_stream_>>>(p);
@@ -820,33 +883,22 @@ class CudaBackend : public Backend {
       ++launches_;
       CK(cudaEventRecord(ev_fork_, side_stream_));   // (re-recorded as the join: the wait above already holds the fork)
     }
-    void* args[] = {&p, &xs};
+    void* args[] = {&p, &l.x};
     // the rows kernel evaluates every row of the batch into the export arrays, one thread per row
-    if (spec_rows_grid_) {
-      CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.rows_kern), dim3(spec_rows_grid_), dim3((unsigned)se.rows_threads), args, 0, st));
+    if (l.rows_grid) {
+      CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.rows_kern), dim3(l.rows_grid), dim3((unsigned)se.rows_threads), args, 0, st));
       ++launches_;
     }
     // persistent CTAs, as many as are resident at once, walk the tiles with a grid stride: the per-CTA set-up (tables, enforcement
     // mask) is paid once per CTA, and where two or more are resident one CTA's copy overlaps another's object walk.  (Launched as the
     // rows kernel's programmatic dependent, so that this set-up overlaps the rows kernel's last blocks, it measured no faster.)
-    CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.kern), dim3(spec_grid), dim3((unsigned)se.threads), args, spec_smem_, st));
+    CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.kern), dim3(spec_grid), dim3((unsigned)se.threads), args, l.spec_smem, st));
     ++launches_;
-    if (spec_units_) CK(cudaStreamWaitEvent(st, ev_fork_, 0));
+    if (l.units) CK(cudaStreamWaitEvent(st, ev_fork_, 0));
     last_kernel_ = "gk_spec_kernel";
-    if (getenv("GK_TRACE_LAUNCH")) {   // (a read-back, so only when tracing)
-      uint32_t nu = 0;
-      CK(cudaMemcpyAsync(&nu, p.unit_count, 4, cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
-      std::vector<uint32_t> u((size_t)nu * 2);
-      if (nu) CK(cudaMemcpy(u.data(), p.units, u.size() * 4, cudaMemcpyDeviceToHost));
-      uint64_t objs = 0, whole = 0;
-      for (uint32_t i = 0; i < nu; ++i) {
-        objs += u[2 * i + 1];
-        whole += u[2 * i + 1] > 1u;
-      }
-      fprintf(stderr, "[spec] handed to the interpreter: %u units (%llu of more than one object), %llu objects, on %u CTAs\n", nu, (unsigned long long)whole,
-              (unsigned long long)objs, grid);
-    }
+    if (getenv("GK_TRACE_LAUNCH"))
+      fprintf(stderr, "[spec] handed to the interpreter: %u units (%llu of more than one object), %llu objects, on %u CTAs\n", l.units,
+              (unsigned long long)l.multi, (unsigned long long)l.handed, grid);
   }
 
   // ---- the specialised kernel: source per constraint-set version (spec_codegen.cpp), compiled by NVRTC when first needed
@@ -969,14 +1021,13 @@ class CudaBackend : public Backend {
     out.words = db->words;
     unsigned long long* totals = d_totals_;
     unsigned long long* err_totals = d_totals_ + std::max(C, 1u);
-    size_t smem = 0;
     uint32_t nerr = 0;
     for (;;) {
-      KParams p = prepare(db, active, db->viol, db->err, totals, err_totals, stream_, &smem);
+      const Launch l = prepare(db, active, db->viol, db->err, totals, err_totals, stream_);
       CK(cudaStreamSynchronize(stream_));
       // the event pair brackets exactly the evaluation kernel
       CK(cudaEventRecord(ev0_, stream_));
-      fire(p, smem, stream_);
+      fire(l);
       CK(cudaEventRecord(ev1_, stream_));
       CK(cudaStreamSynchronize(stream_));
       CK(cudaMemcpy(&nerr, d_scalars_, 4, cudaMemcpyDeviceToHost));
@@ -1024,15 +1075,17 @@ class CudaBackend : public Backend {
     }
     out.errlist.resize((size_t)nerr * 3);
     if (nerr) CK(cudaMemcpy(out.errlist.data(), d_errlist_, (size_t)nerr * 12, cudaMemcpyDeviceToHost));
-    if (copy_back) {
-      out.viol.resize((size_t)db->n * db->words);
-      out.err.resize((size_t)db->n * db->words);
-      if (db->n) {
-        CK(cudaMemcpyAsync(out.viol.data(), db->viol, out.viol.size() * 4, cudaMemcpyDeviceToHost, stream_));
-        CK(cudaMemcpyAsync(out.err.data(), db->err, out.err.size() * 4, cudaMemcpyDeviceToHost, stream_));
-        CK(cudaStreamSynchronize(stream_));
-      }
-    }
+    if (copy_back) copy_planes(*db, out);
+  }
+
+  // a batch's result planes into `out`
+  void copy_planes(const DevBatch& db, EvalOut& out) {
+    out.viol.resize((size_t)db.n * db.words);
+    out.err.resize((size_t)db.n * db.words);
+    if (!db.n) return;
+    CK(cudaMemcpyAsync(out.viol.data(), db.viol, out.viol.size() * 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(out.err.data(), db.err, out.err.size() * 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
   }
 
   // ---- device ingest (ingest_core.h / ingest_kernels.cuh): raw JSON blob -> resident columnar batch
@@ -1147,16 +1200,13 @@ class CudaBackend : public Backend {
     bytes.assign((size_t)off.back(), '\0');
     const uint32_t nspans = (uint32_t)(spans.size() / 3);
     if (!nspans || bytes.empty()) return;
-    unsigned long long* d_spans = nullptr;
-    uint8_t* d_out = nullptr;
-    dmalloc(&d_spans, spans.size() * 8);
-    dmalloc(&d_out, bytes.size());
+    Temps temps(this);
+    auto* d_spans = temps.take<unsigned long long>(spans.size() * 8);
+    auto* d_out = temps.take<uint8_t>(bytes.size());
     CK(cudaMemcpyAsync(d_spans, spans.data(), spans.size() * 8, cudaMemcpyHostToDevice, stream_));
     gk_gather_kernel<<<std::min<uint32_t>(nspans, 4096u), 128, 0, stream_>>>(d_out, ks->in.blob, d_spans, nspans);
     ++launches_;
     CK(cudaMemcpyAsync(&bytes[0], d_out, bytes.size(), cudaMemcpyDeviceToHost, stream_));
-    dfree(d_spans);
-    dfree(d_out);
     CK(cudaStreamSynchronize(stream_));
     CK(cudaGetLastError());
   }
@@ -1252,11 +1302,7 @@ class CudaBackend : public Backend {
     uint32_t clanes = 1;
     if (const char* ev = getenv("GK_INGEST_COL_LANES")) clanes = std::max(1, std::min(32, atoi(ev)));
     while (clanes & (clanes - 1)) --clanes;
-    cudaEvent_t e0, e1, e2, e3;
-    CK(cudaEventCreate(&e0));
-    CK(cudaEventCreate(&e1));
-    CK(cudaEventCreate(&e2));
-    CK(cudaEventCreate(&e3));
+    Event e0, e1, e2, e3;
     CK(cudaEventRecord(e0, stream_));
     const GkIngestIn src = acquire();
     // ---- back scratch: header counters + scratch flags, totals, scan block sums, miss list, the pointer tables of the count phase
@@ -1296,20 +1342,7 @@ class CudaBackend : public Backend {
     outc.row_rec = reinterpret_cast<GkRowRec* const*>(d_s + o_prec);
     std::vector<uint64_t> h_prec(NS, 0);
     std::vector<uint32_t*> d_cnt(NS, nullptr), d_coll(NS, nullptr), d_blen(xh.nbytecols, nullptr);
-    std::vector<void*> temps;   // stream-ordered allocations of this call
-    struct TempGuard {
-      CudaBackend* be;
-      std::vector<void*>* v;
-      ~TempGuard() {
-        for (void* p2 : *v) be->dfree(p2);
-      }
-    } temp_guard{this, &temps};
-    auto talloc = [&](size_t bytes) {
-      uint8_t* p2 = nullptr;
-      dmalloc(&p2, bytes);
-      temps.push_back(p2);
-      return p2;
-    };
+    Temps temps(this);
     CK(cudaEventRecord(e1, stream_));
     std::vector<uint32_t> total(NS, 0), htot(GK_CNT_EXTRA, 0), btot(xh.nbytecols, 0);
     total[0] = n;
@@ -1326,8 +1359,8 @@ class CudaBackend : public Backend {
         for (uint32_t t = 1; t < NS; ++t) {
           if (depth[t] != d) continue;
           const uint32_t prows = total[xh.scopes[t].parent];
-          d_cnt[t] = reinterpret_cast<uint32_t*>(talloc(((size_t)prows + 1) * 4));
-          d_coll[t] = reinterpret_cast<uint32_t*>(talloc(((size_t)prows + 1) * 4));
+          d_cnt[t] = temps.take<uint32_t>(((size_t)prows + 1) * 4);
+          d_coll[t] = temps.take<uint32_t>(((size_t)prows + 1) * 4);
           if (prows) {
             gk_scope_count_kernel<<<blocks(prows), kIngestThreads, 0, stream_>>>(xp, in, outc, t, prows, d_cnt[t], d_coll[t]);
             ++launches_;
@@ -1341,7 +1374,7 @@ class CudaBackend : public Backend {
         for (uint32_t t = 1; t < NS; ++t) {
           if (depth[t] != d) continue;
           total[t] = hbuf[GK_CNT_EXTRA + t];
-          h_prec[t] = reinterpret_cast<uint64_t>(talloc(((size_t)total[t] + 1) * sizeof(GkRowRec)));
+          h_prec[t] = reinterpret_cast<uint64_t>(temps.take(((size_t)total[t] + 1) * sizeof(GkRowRec)));
           any = true;
         }
         if (!any) continue;
@@ -1359,7 +1392,7 @@ class CudaBackend : public Backend {
         const GkXCol& xc = xh.cols[ci];
         if (!(xc.enc & GK_ENC_BYTES)) continue;
         const uint32_t rows = total[xc.scope];
-        d_blen[xc.bytes_slot] = reinterpret_cast<uint32_t*>(talloc(((size_t)rows + 1) * 4));
+        d_blen[xc.bytes_slot] = temps.take<uint32_t>(((size_t)rows + 1) * 4);
         if (rows) {
           gk_bcol_len_kernel<<<blocks(rows), kIngestThreads, 0, stream_>>>(xp, in, outc, ci, rows, d_blen[xc.bytes_slot]);
           ++launches_;
@@ -1492,7 +1525,7 @@ class CudaBackend : public Backend {
     out.bytes = reinterpret_cast<uint8_t* const*>(A + a_pbytes);
     out.head = reinterpret_cast<uint32_t* const*>(A + a_phead);
     out.row_rec = outc.row_rec;   // (the row handles of the count phase)
-    unsigned long long* d_mm = reinterpret_cast<unsigned long long*>(talloc(64));
+    unsigned long long* d_mm = temps.take<unsigned long long>(64);
     {
       const unsigned long long init[2] = {~0ull, 0ull};
       push_small(d_mm, init, 16);
@@ -1552,8 +1585,8 @@ class CudaBackend : public Backend {
         std::vector<uint8_t> args(gk_compact_miss_spans(hmiss.data(), m, spans) + 1);
         const uint32_t nspans = (uint32_t)(spans.size() / 3);
         if (nspans) {
-          auto* d_spans = reinterpret_cast<unsigned long long*>(talloc(spans.size() * 8));
-          uint8_t* d_args = talloc(args.size());
+          auto* d_spans = temps.take<unsigned long long>(spans.size() * 8);
+          auto* d_args = temps.take<uint8_t>(args.size());
           CK(cudaMemcpyAsync(d_spans, spans.data(), spans.size() * 8, cudaMemcpyHostToDevice, stream_));
           gk_gather_kernel<<<std::min<uint32_t>(nspans, 4096u), 128, 0, stream_>>>(d_args, in.blob, d_spans, nspans);
           ++launches_;
@@ -1651,10 +1684,6 @@ class CudaBackend : public Backend {
               n, B / 1e6, a, b, (unsigned long long)total_miss, lut_ms, d,
               std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - T0).count(), db->bytes / 1e6);
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaEventDestroy(e2);
-    cudaEventDestroy(e3);
     guard.release();
     return db;
   }
@@ -1720,36 +1749,16 @@ class CudaBackend : public Backend {
     if (device_ms) *device_ms = 0.f;
     if (!n || !C || !words) return;
     if (!db->gvk) throw BackendError{"audit candidates: the batch holds no apiVersion / kind hashes"};
-    std::vector<void*> temps;
-    struct Free {
-      CudaBackend* be;
-      std::vector<void*>& t;
-      ~Free() {
-        for (void* p : t) be->dfree(p);
-      }
-    } free_temps{this, temps};
-    auto take = [&](size_t bytes) {
-      void* p = nullptr;
-      dmalloc(&p, bytes);
-      temps.push_back(p);
-      return p;
-    };
+    Temps temps(this);
     uint32_t cap = 1024;
     while (cap < 2 * n) cap <<= 1;
     const uint32_t mask = cap - 1, T = 256, grid = std::min<uint32_t>((n + T - 1) / T, (uint32_t)sms_ * 16);
-    auto* keys = static_cast<unsigned long long*>(take((size_t)cap * 8));
-    auto* rep = static_cast<uint32_t*>(take((size_t)cap * 4));
-    auto* d_cnt = static_cast<uint32_t*>(take(64));
-    auto* d_list = static_cast<uint32_t*>(take((size_t)2 * n * 4));
-    auto* d_viol = static_cast<uint32_t*>(take((size_t)n * words * 4));
-    cudaEvent_t e0, e1, e2, e3;
-    for (cudaEvent_t* e : {&e0, &e1, &e2, &e3}) CK(cudaEventCreate(e));
-    struct Ev {
-      cudaEvent_t* e[4];
-      ~Ev() {
-        for (auto x : e) cudaEventDestroy(*x);
-      }
-    } ev_guard{{&e0, &e1, &e2, &e3}};
+    auto* keys = temps.take<unsigned long long>((size_t)cap * 8);
+    auto* rep = temps.take<uint32_t>((size_t)cap * 4);
+    auto* d_cnt = temps.take<uint32_t>(64);
+    auto* d_list = temps.take<uint32_t>((size_t)2 * n * 4);
+    auto* d_viol = temps.take<uint32_t>((size_t)n * words * 4);
+    Event e0, e1, e2, e3;
     CK(cudaMemcpyAsync(d_viol, viol, (size_t)n * words * 4, cudaMemcpyHostToDevice, stream_));
     CK(cudaEventRecord(e0, stream_));
     CK(cudaMemsetAsync(keys, 0, (size_t)cap * 8, stream_));
@@ -1782,10 +1791,10 @@ class CudaBackend : public Backend {
       pairs[2 * i] = list[2 * tri[i].j];
       pairs[2 * i + 1] = r;
     }
-    auto* gr = static_cast<uint32_t*>(take((size_t)n * 4));
-    auto* perm = static_cast<uint32_t*>(take((size_t)n * 4));
-    auto* head = static_cast<uint32_t*>(take((size_t)n * 4));
-    auto* rank = static_cast<uint32_t*>(take((size_t)n * 4));
+    auto* gr = temps.take<uint32_t>((size_t)n * 4);
+    auto* perm = temps.take<uint32_t>((size_t)n * 4);
+    auto* head = temps.take<uint32_t>((size_t)n * 4);
+    auto* rank = temps.take<uint32_t>((size_t)n * 4);
     CK(cudaEventRecord(e2, stream_));
     if (m) {
       CK(cudaMemcpyAsync(d_list, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, stream_));
@@ -1796,15 +1805,15 @@ class CudaBackend : public Backend {
     size_t sort_bytes = 0, scan_bytes = 0;
     CK(cub::DeviceMergeSort::SortKeys(nullptr, sort_bytes, perm, (int64_t)n, less, stream_));
     CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, head, rank, (int64_t)n, stream_));
-    void* cub_tmp = take(std::max(sort_bytes, scan_bytes));
+    void* cub_tmp = temps.take(std::max(sort_bytes, scan_bytes));
     CK(cub::DeviceMergeSort::SortKeys(cub_tmp, sort_bytes, perm, (int64_t)n, less, stream_));
     gk_id_heads_kernel<<<grid, T, 0, stream_>>>(perm, n, less, head);
     CK(cub::DeviceScan::InclusiveSum(cub_tmp, scan_bytes, head, gr, (int64_t)n, stream_));   // (gr is free again: the sort is done)
     gk_id_scatter_kernel<<<grid, T, 0, stream_>>>(perm, gr, n, rank);
     const uint32_t nb = (n + kSelChunk - 1) / kSelChunk;
-    auto* cnt = static_cast<uint32_t*>(take((size_t)nb * C * 4));
-    auto* thr = static_cast<uint32_t*>(take((size_t)C * 4));
-    auto* d_cand = static_cast<uint32_t*>(take((size_t)n * words * 4));
+    auto* cnt = temps.take<uint32_t>((size_t)nb * C * 4);
+    auto* thr = temps.take<uint32_t>((size_t)C * 4);
+    auto* d_cand = temps.take<uint32_t>((size_t)n * words * 4);
     if ((size_t)C * 4 > max_smem_) throw BackendError{"audit candidates: too many constraints for one block's counters"};
     if ((size_t)C * 4 > 48 * 1024) CK(cudaFuncSetAttribute(gk_sel_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(C * 4)));
     gk_sel_count_kernel<<<nb, 256, (size_t)C * 4, stream_>>>(perm, d_viol, n, words, C, cnt);
@@ -1916,18 +1925,8 @@ class CudaBackend : public Backend {
     auto* db = static_cast<DevBatch*>(b);
     std::lock_guard<std::mutex> l(mu_);
     CK(cudaSetDevice(device_));
-    size_t smem = 0;
-    cudaStream_t st = static_cast<cudaStream_t>(dst.stream);
-    KParams p = prepare(db, active, static_cast<uint32_t*>(dst.viol), static_cast<uint32_t*>(dst.err), static_cast<unsigned long long*>(dst.totals),
-                        static_cast<unsigned long long*>(dst.err_totals), st, &smem);
-    if (dst.npeers > GK_MAX_PEERS) throw BackendError{"too many peers for the fused exchange"};
-    p.npeers = dst.npeers;
-    p.tot_stride = dst.tot_stride;
-    for (uint32_t q = 0; q < dst.npeers; ++q) {
-      p.peer_viol[q] = reinterpret_cast<uint32_t*>(dst.peer_viol[q]);
-      p.peer_tot[q] = reinterpret_cast<unsigned long long*>(dst.peer_tot[q]);
-    }
-    fire(p, smem, st);
+    fire(prepare(db, active, static_cast<uint32_t*>(dst.viol), static_cast<uint32_t*>(dst.err), static_cast<unsigned long long*>(dst.totals),
+                 static_cast<unsigned long long*>(dst.err_totals), static_cast<cudaStream_t>(dst.stream), dst));
   }
 
   // Generator selection: the page's distinct apiVersion / kind hashes into a device table (as audit_candidates finds them), decided on
@@ -1942,35 +1941,15 @@ class CudaBackend : public Backend {
     if (device_ms) *device_ms = 0.f;
     if (!n) return;
     if (!db->gvk) throw BackendError{"select generators: the batch holds no apiVersion / kind hashes"};
-    std::vector<void*> temps;
-    struct Free {
-      CudaBackend* be;
-      std::vector<void*>& t;
-      ~Free() {
-        for (void* p : t) be->dfree(p);
-      }
-    } free_temps{this, temps};
-    auto take = [&](size_t bytes) {
-      void* p = nullptr;
-      dmalloc(&p, bytes);
-      temps.push_back(p);
-      return p;
-    };
+    Temps temps(this);
     uint32_t cap = 1024;
     while (cap < 2 * n) cap <<= 1;
     const uint32_t mask = cap - 1, T = 256, grid = std::min<uint32_t>((n + T - 1) / T, (uint32_t)sms_ * 16);
-    auto* keys = static_cast<unsigned long long*>(take((size_t)cap * 8));
-    auto* rep = static_cast<uint32_t*>(take((size_t)cap * 4));
-    auto* d_cnt = static_cast<uint32_t*>(take(64));
-    auto* d_list = static_cast<uint32_t*>(take((size_t)2 * n * 4));
-    cudaEvent_t e0, e1, e2, e3;
-    for (cudaEvent_t* e : {&e0, &e1, &e2, &e3}) CK(cudaEventCreate(e));
-    struct Ev {
-      cudaEvent_t* e[4];
-      ~Ev() {
-        for (auto x : e) cudaEventDestroy(*x);
-      }
-    } ev_guard{{&e0, &e1, &e2, &e3}};
+    auto* keys = temps.take<unsigned long long>((size_t)cap * 8);
+    auto* rep = temps.take<uint32_t>((size_t)cap * 4);
+    auto* d_cnt = temps.take<uint32_t>(64);
+    auto* d_list = temps.take<uint32_t>((size_t)2 * n * 4);
+    Event e0, e1, e2, e3;
     CK(cudaEventRecord(e0, stream_));
     CK(cudaMemsetAsync(keys, 0, (size_t)cap * 8, stream_));
     CK(cudaMemsetAsync(rep, 0xff, (size_t)cap * 4, stream_));
@@ -1991,9 +1970,9 @@ class CudaBackend : public Backend {
       if (wanted(g, v, k)) pairs.insert(pairs.end(), {list[2 * j], 1u});
     }
     const uint32_t np = (uint32_t)(pairs.size() / 2);
-    auto* mark = static_cast<uint8_t*>(take(n));
-    auto* idx = static_cast<uint32_t*>(take((size_t)n * 4));
-    auto* d_sel = static_cast<uint32_t*>(take((size_t)n * 4));
+    auto* mark = temps.take<uint8_t>(n);
+    auto* idx = temps.take<uint32_t>((size_t)n * 4);
+    auto* d_sel = temps.take<uint32_t>((size_t)n * 4);
     CK(cudaEventRecord(e2, stream_));
     CK(cudaMemsetAsync(rep, 0, (size_t)cap * 4, stream_));   // (rep is free again: now the pick flag per slot)
     if (np) {
@@ -2003,7 +1982,7 @@ class CudaBackend : public Backend {
     gk_gen_mark_kernel<<<grid, T, 0, stream_>>>(db->gvk, n, keys, rep, mask, mark, idx);
     size_t sel_bytes = 0;
     CK(cub::DeviceSelect::Flagged(nullptr, sel_bytes, idx, mark, d_sel, d_cnt, (int64_t)n, stream_));
-    CK(cub::DeviceSelect::Flagged(take(sel_bytes), sel_bytes, idx, mark, d_sel, d_cnt, (int64_t)n, stream_));
+    CK(cub::DeviceSelect::Flagged(temps.take(sel_bytes), sel_bytes, idx, mark, d_sel, d_cnt, (int64_t)n, stream_));
     CK(cudaEventRecord(e3, stream_));
     uint32_t g = 0;
     CK(cudaMemcpyAsync(&g, d_cnt, 4, cudaMemcpyDeviceToHost, stream_));
@@ -2113,15 +2092,7 @@ class CudaBackend : public Backend {
       out.totals[c] += t[c];
       out.err_totals[c] += t[C + c];
     }
-    if (copy_back) {
-      out.viol.resize((size_t)db->n * db->words);
-      out.err.resize((size_t)db->n * db->words);
-      if (db->n) {
-        CK(cudaMemcpyAsync(out.viol.data(), db->viol, out.viol.size() * 4, cudaMemcpyDeviceToHost, stream_));
-        CK(cudaMemcpyAsync(out.err.data(), db->err, out.err.size() * 4, cudaMemcpyDeviceToHost, stream_));
-        CK(cudaStreamSynchronize(stream_));
-      }
-    }
+    if (copy_back) copy_planes(*db, out);
   }
 
   void fold_into(void* res, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off, const std::vector<uint32_t>& active,
@@ -2130,23 +2101,15 @@ class CudaBackend : public Backend {
     auto* r = static_cast<DevBatch*>(res);
     std::lock_guard<std::mutex> l(mu_);
     CK(cudaSetDevice(device_));
-    if (dst.npeers > GK_MAX_PEERS || (dst.npeers && dst.rank >= dst.npeers)) throw BackendError{"fold: bad peer addressing"};
+    GkFoldArgs a = fold_args(*r);
+    set_peers(a, dst);
     const uint32_t C = prog_.nconstraints;
     cudaStream_t st = static_cast<cudaStream_t>(dst.stream);
     // the resultants into their own planes (their totals are not the caller's)
-    size_t smem = 0;
-    KParams p = prepare(r, active, r->viol, r->err, r->fold_tot, r->fold_tot + std::max(C, 1u), st, &smem);
-    fire(p, smem, st);
-    GkFoldArgs a = fold_args(*r);
+    fire(prepare(r, active, r->viol, r->err, r->fold_tot, r->fold_tot + std::max(C, 1u), st));
     a.sviol = dst.npeers ? reinterpret_cast<const uint32_t*>(dst.peer_viol[dst.rank]) : static_cast<const uint32_t*>(dst.viol);
     a.serr = a.derr = static_cast<uint32_t*>(dst.err);
     a.dviol = dst.npeers ? nullptr : static_cast<uint32_t*>(dst.viol);
-    a.npeers = dst.npeers;
-    a.tot_stride = dst.tot_stride;
-    for (uint32_t q = 0; q < dst.npeers; ++q) {
-      a.peer_viol[q] = reinterpret_cast<uint32_t*>(dst.peer_viol[q]);
-      a.peer_tot[q] = reinterpret_cast<unsigned long long*>(dst.peer_tot[q]);
-    }
     a.totals = static_cast<unsigned long long*>(dst.totals);
     a.err_totals = static_cast<unsigned long long*>(dst.err_totals);
     launch_fold(a, st);
@@ -2222,11 +2185,6 @@ class CudaBackend : public Backend {
   int spec_rows_minb_ = getenv("GK_SPEC_ROWS_MINB") ? std::max(1, atoi(getenv("GK_SPEC_ROWS_MINB"))) : 6;   // 256 x 6: a 40-register cap, no spill at config 2 (DESIGN 5a)
   uint32_t* d_spec_x_ = nullptr;   // the export arrays (SpecSource::export_bytes), grow-only
   size_t spec_x_bytes_ = 0;
-  uint32_t spec_rows_grid_ = 0;    // blocks of the next rows-kernel launch (set with spec_next_)
-  bool spec_next_ = false;
-  uint32_t spec_units_ = 0;   // units the interpreter evaluates beside the next launch of the generated kernel (set with spec_next_)
-  size_t spec_smem_ = 0;      // dynamic shared memory of the next launch of the generated kernel (set with spec_next_)
-  int spec_per_sm_ = 1;       // its resident CTAs per SM at that size
   size_t optin_smem_ = 0;     // the device's per-CTA shared-memory limit
   void* pinned_ = nullptr;
   size_t pinned_bytes_ = 0;

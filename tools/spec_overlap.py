@@ -48,7 +48,7 @@ def profile():
         blob = Wl.PyBlob(docs)
     rb = drv.upload_blob(blob)
 
-    # one traced evaluation (a read-back of the unit list), outside the profiled ones
+    # one traced evaluation, outside the profiled ones
     err = tempfile.TemporaryFile()
     saved = os.dup(2)
     os.dup2(err.fileno(), 2)

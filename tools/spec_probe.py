@@ -8,7 +8,7 @@ launch time (both kernels) of several build variants (threads per CTA x minimum 
 A variant is TILExMINB[@ROWSxMINB][:SWITCH+SWITCH]: the shape of gk_spec_kernel, optionally of gk_spec_rows_kernel, and measurement
 switches of the text (GENERIC = spec.match through the shared gk_match(); otherwise -DGK_SPEC_X_<SWITCH>: NOMATCH, STAGEONLY).
 With --handover, every variant runs once per value of GK_HANDOVER_MAX (program.h; 0 = every tile with a wide object handed over
-whole).  Each line reports the units handed to the interpreter and the objects they hold (read back once, outside the timed loop).
+whole).  Each line reports the units handed to the interpreter and the objects they hold (traced once, outside the timed loop).
 """
 import argparse
 import json
@@ -71,7 +71,7 @@ def run(label, env):
     drv = engine()
     drv.pin_blob(blob)
     rb = drv.upload_blob(blob)
-    # the first evaluation builds the kernel and, traced, reports the hand-over (a read-back): outside the timed launches below
+    # the first evaluation builds the kernel and, traced, reports the hand-over: outside the timed launches below
     err = tempfile.TemporaryFile()
     saved = os.dup(2)
     os.dup2(err.fileno(), 2)
