@@ -66,6 +66,10 @@ struct DevBatch {
   uint32_t nunits = 0;               // the plan's unit count
   uint32_t multi = 0;                // of those, units of more than one object (a whole tile's wide objects)
   uint64_t handed = 0;               // the objects those units cover
+  // the offset image the plan writes beside it (SpecSource::image_stride): img_stride values per tile, grown (never shrunk)
+  uint16_t* d_img = nullptr;
+  size_t img_bytes = 0;
+  uint32_t img_stride = 0;
   // the netlist with every slot id replaced by the slot's word offset in this batch's shared-memory slot area
   GkOp* d_ops = nullptr;
   uint32_t* d_pool = nullptr;
@@ -684,6 +688,7 @@ class CudaBackend : public Backend {
     dfree(db->fold_tot);
     dfree(db->d_units);
     dfree(db->d_whole);
+    dfree(db->d_img);
     dfree(db->d_ops);
     dfree(db->d_pool);
     dfree(db->d_outs);
@@ -700,6 +705,8 @@ class CudaBackend : public Backend {
     cudaStream_t st = nullptr;
     SpecEntry* spec = nullptr;   // the generated kernel, or null: the interpreter alone
     uint32_t* x = nullptr;       // its export arrays
+    const uint16_t* img = nullptr;   // the batch's offset image, img_stride values per tile
+    uint32_t img_stride = 0;
     size_t spec_smem = 0;        // its dynamic shared memory per CTA
     int spec_per_sm = 1;         // its resident CTAs per SM at that size
     uint32_t rows_grid = 0;      // blocks of the rows kernel
@@ -763,11 +770,12 @@ class CudaBackend : public Backend {
       SpecEntry& se = *spec_cur_;
       // The generated kernel stages the largest tile's rows in shared memory: one bit per row per export plane of a scope that has
       // atoms, where the interpreter holds one bit per row per live slot.  A scope with many rows in a tile can therefore need more
-      // than the device allows while the interpreter fits: that batch is interpreted.
+      // than the device allows while the interpreter fits: that batch is interpreted.  So is a batch with a tile of more rows in a
+      // nested scope than the offset image's 16-bit values hold.
       // (the rows read the batch's type words as the text lays them out: both come from gk_tw_layout over the same columns)
       if (!(se.src.tw == db->tw)) throw BackendError{"batch type words are laid out for another column table"};
       l.spec_smem = se.src.smem + se.src.stage_bytes(db->cap);
-      bool run = l.spec_smem <= se.max_smem;
+      bool run = l.spec_smem <= se.max_smem && se.src.image_fits(db->cap);
       l.spec_per_sm = 0;   // resident CTAs per SM: the persistent grid of fire()
       if (run && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&l.spec_per_sm, reinterpret_cast<const void*>(se.kern), se.threads, l.spec_smem) != cudaSuccess) {
         cudaGetLastError();
@@ -777,10 +785,24 @@ class CudaBackend : public Backend {
       // The hand-over plan depends on the batch's CSR offsets, which never change, and on the generated text: made by the first
       // evaluation of the batch with this constraint set, here, and kept, with its unit counts and the objects they cover on the host.
       // (It reads every offset array the netlist uses: at config 2 about as long as the interpreter's units take, so planning on
-      // every evaluation would give back most of the overlap.)
+      // every evaluation would give back most of the overlap.)  The same pass writes the batch's offset image, which the tile kernel
+      // stages instead of reading those arrays again.
       if (run && db->planned != se.version && p.ntiles) {
+        db->img_stride = se.src.image_stride(db->cap);
+        const size_t ib = (size_t)p.ntiles * db->img_stride * 2;
+        if (ib > db->img_bytes) {
+          CK(cudaStreamSynchronize(st));   // (an evaluation still in flight may be reading the old image)
+          dfree(db->d_img);
+          db->d_img = nullptr;
+          db->img_bytes = 0;
+          dmalloc(&db->d_img, ib);
+          CK(cudaStreamSynchronize(stream_));
+          db->img_bytes = ib;
+        }
+        if (getenv("GK_TRACE_LAUNCH"))
+          fprintf(stderr, "[spec] offset image: %zu bytes, %u bytes per tile x %u tiles\n", ib, db->img_stride * 2, p.ntiles);
         CK(cudaMemsetAsync(p.unit_count, 0, 4, st));
-        void* args[] = {&p};
+        void* args[] = {&p, &db->d_img, &db->img_stride};
         CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.plan_kern), dim3(p.ntiles), dim3(256), args, 0, st));
         ++launches_;
         CK(cudaMemcpyAsync(&db->nunits, p.unit_count, 4, cudaMemcpyDeviceToHost, st));
@@ -811,6 +833,8 @@ class CudaBackend : public Backend {
       if (run) {
         l.spec = &se;
         l.x = d_spec_x_;
+        l.img = db->d_img;
+        l.img_stride = db->img_stride;
         l.rows_grid = se.src.rows_blocks(db->rows, (uint32_t)se.rows_threads);
         l.units = db->nunits;
         l.multi = db->multi;
@@ -883,10 +907,11 @@ class CudaBackend : public Backend {
       ++launches_;
       CK(cudaEventRecord(ev_fork_, side_stream_));   // (re-recorded as the join: the wait above already holds the fork)
     }
-    void* args[] = {&p, &l.x};
-    // the rows kernel evaluates every row of the batch into the export arrays, one thread per row
+    void* args[] = {&p, &l.x, &l.img, &l.img_stride};
+    // the rows kernel evaluates every row of the batch into the export arrays, one thread per row (its parameters: the first two)
     if (l.rows_grid) {
-      CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.rows_kern), dim3(l.rows_grid), dim3((unsigned)se.rows_threads), args, 0, st));
+      void* rows_args[] = {&p, &l.x};
+      CK(cudaLaunchKernel(reinterpret_cast<const void*>(se.rows_kern), dim3(l.rows_grid), dim3((unsigned)se.rows_threads), rows_args, 0, st));
       ++launches_;
     }
     // persistent CTAs, as many as are resident at once, walk the tiles with a grid stride: the per-CTA set-up (tables, enforcement

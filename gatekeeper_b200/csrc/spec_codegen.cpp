@@ -38,7 +38,9 @@ std::string hx(uint32_t v) {
 // the fixed part: launch wrapper (device) / per-object entry point (host test build)
 const char* kWrapper = R"GKSRC(
 #ifndef GK_SPEC_HOST
-extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_spec_kernel(const __grid_constant__ GkKParams p, const uint32_t* __restrict__ xs) {
+// xs: the export planes (gk_spec_rows_kernel); img: the offset image, a run of img_stride values per tile (gk_spec_plan_kernel)
+extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_spec_kernel(const __grid_constant__ GkKParams p, const uint32_t* __restrict__ xs,
+                                                                                          const uint16_t* __restrict__ img, const uint32_t img_stride) {
   extern __shared__ uint4 gk_smem4[];
   unsigned char* smem = reinterpret_cast<unsigned char*>(gk_smem4);
   const uint32_t NC = p.batch.ncols, NS = p.batch.nscopes;
@@ -79,7 +81,7 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
     // phase 1: the copy of the tile's exports and offsets, every thread of the CTA; phase 2: its objects, one per thread.  (The
     // barrier at the end of the tile keeps the next tile's copy from overwriting what the last objects of this one still read.)
     const uint32_t* tl = p.tile_lo + (size_t)t * NS;
-    gk_spec_stage(p.batch, scopes, xs, tl, tl + NS, stg, threadIdx.x, blockDim.x);
+    gk_spec_stage(p.batch, scopes, xs, img + (size_t)t * img_stride, tl, tl + NS, stg, threadIdx.x, blockDim.x);
     __syncthreads();
 #ifdef GK_SPEC_X_STAGEONLY   /* (measurement only: the staging of every tile without the object walk; results differ) */
     for (uint32_t base = nobj; base < nobj; base += blockDim.x) {
@@ -149,9 +151,12 @@ extern "C" __global__ void __launch_bounds__(GK_SPEC_THREADS, GK_SPEC_MINB) gk_s
 
 // The hand-over plan, before any row is evaluated: one CTA per tile finds the tile's wide objects from the CSR offsets
 // (gk_spec_wide) and lists them for the interpreter -- each alone, or the whole tile when it has more than GK_HANDOVER_MAX
-// (gk_spec_tile_whole) -- and sets the tile's whole flag, which gk_spec_kernel reads.
-extern "C" __global__ void gk_spec_plan_kernel(const __grid_constant__ GkKParams p) {
+// (gk_spec_tile_whole) -- and sets the tile's whole flag, which gk_spec_kernel reads.  It also writes the tile's run of the offset
+// image (gk_spec_offsets), which gk_spec_kernel stages.
+extern "C" __global__ void gk_spec_plan_kernel(const __grid_constant__ GkKParams p, uint16_t* __restrict__ img, const uint32_t img_stride) {
   const uint32_t t = blockIdx.x, obj0 = t * p.tile, nobj = min(p.tile, p.batch.n - obj0);
+  const uint32_t* tl = p.tile_lo + (size_t)t * p.batch.nscopes;
+  gk_spec_offsets(p.batch.scopes, tl, tl + p.batch.nscopes, img + (size_t)t * img_stride, threadIdx.x, blockDim.x);
   uint32_t nwide = 0u;
   for (uint32_t base = 0; base < nobj; base += blockDim.x) {
     const uint32_t o = base + threadIdx.x;
@@ -181,13 +186,39 @@ extern "C" __global__ void gk_spec_plan_kernel(const __grid_constant__ GkKParams
 #include <string>
 // TEST-ONLY host build: the hand-over plan of gk_spec_plan_kernel for tiles of `tile` objects, tile after tile and a tile's
 // objects in order (the kernel appends them in any order).  Fills units (capacity: 2 per object) and whole (one per tile); returns
-// the units.
+// the units.  Also, into `im`, the offset image of those tiles as the kernel writes it: `stride` values per tile
+// (gk_spec_image_stride of the largest tile's rows per scope, the tile itself in scope 0, as the backend sizes it), a value no run
+// covers poisoned; `fits` as the backend decides whether the batch may run the generated kernel (gk_spec_image_fits).
 #ifndef GK_SPEC_HOST_PLAN_TILE
 #define GK_SPEC_HOST_PLAN_TILE 512u   /* the device's tile (tile_kernel.cuh GK_TILE) */
 #endif
-static uint32_t gk_spec_host_plan(const GkBatch& B, uint32_t tile, std::vector<uint32_t>& units, std::vector<uint32_t>& whole) {
+struct GkSpecHostImage {
+  std::vector<uint16_t> img;
+  std::vector<uint32_t> lo, hi;   // [tiles * GK_SPEC_NS] each tile's first row and end per scope (the nested scopes and scope 0)
+  uint32_t stride = 0u;
+  bool fits = true;
+};
+static uint32_t gk_spec_host_plan(const GkBatch& B, uint32_t tile, std::vector<uint32_t>& units, std::vector<uint32_t>& whole, GkSpecHostImage& im) {
   units.clear();
   whole.assign((B.n + tile - 1u) / tile, 0u);
+  const size_t NT = whole.size();
+  im.lo.assign(NT * GK_SPEC_NS, 0u);
+  im.hi.assign(NT * GK_SPEC_NS, 0u);
+  std::vector<uint32_t> cap(GK_SPEC_NS, 0u);
+  for (size_t t = 0; t < NT; ++t) {
+    uint32_t* lo = im.lo.data() + t * GK_SPEC_NS;
+    uint32_t* hi = im.hi.data() + t * GK_SPEC_NS;
+    lo[0] = (uint32_t)t * tile;
+    hi[0] = B.n - lo[0] < tile ? B.n : lo[0] + tile;
+    gk_spec_tile_rows(B.scopes, lo, hi);
+    for (uint32_t s = 0; s < GK_SPEC_NS; ++s) cap[s] = hi[s] - lo[s] > cap[s] ? hi[s] - lo[s] : cap[s];
+  }
+  cap[0] = tile;
+  im.stride = gk_spec_image_stride(cap.data());
+  im.fits = gk_spec_image_fits(cap.data());
+  im.img.assign(NT * im.stride, 0xbeefu);
+  for (size_t t = 0; t < NT; ++t)
+    gk_spec_offsets(B.scopes, im.lo.data() + t * GK_SPEC_NS, im.hi.data() + t * GK_SPEC_NS, im.img.data() + t * im.stride, 0u, 1u);
   for (uint32_t t = 0; t < whole.size(); ++t) {
     const uint32_t obj0 = t * tile, nobj = B.n - obj0 < tile ? B.n - obj0 : tile;
     uint32_t nwide = 0u;
@@ -233,6 +264,21 @@ extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint
   for (uint32_t w = 0; w < GK_SPEC_W; ++w) vw[w] = ew[w] = actw[w] = 0u;
   for (uint32_t c = 0; c < GK_SPEC_C; ++c)
     if (p->active[c]) actw[c >> 5] |= 1u << (c & 31u);
+  // the batch's offset image for the tiles below, made again at its first object (the plan kernel writes it once per batch); a batch
+  // whose tile rows do not fit it is the interpreter's: every object is handed over
+  struct Image {
+    const void* flags = nullptr;
+    uint32_t n = 0;
+    GkSpecHostImage im;
+  };
+  static thread_local Image ki;
+  if (obj == 0u || ki.flags != (const void*)p->batch.flags || ki.n != p->batch.n) {
+    std::vector<uint32_t> u, wh;
+    gk_spec_host_plan(p->batch, GK_SPEC_HOST_TILE, u, wh, ki.im);
+    ki.flags = p->batch.flags;
+    ki.n = p->batch.n;
+  }
+  if (!ki.im.fits) return 1;
   struct Tile {
     const void* flags = nullptr;
     uint32_t n = 0, t = 0xffffffffu;
@@ -251,7 +297,8 @@ extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint
     k.stg.assign(gk_spec_stage_words(k.lo.data(), k.hi.data()), 0xdeadbeefu);   // (poisoned: a word the staging misses shows)
     k.x.assign(gk_spec_export_words(B), 0xdeadbeefu);
     gk_spec_host_rows(p, k.lo.data(), k.hi.data(), k.x.data());
-    for (uint32_t tid = 0; tid < 3u; ++tid) gk_spec_stage(B, B.scopes, k.x.data(), k.lo.data(), k.hi.data(), k.stg.data(), tid, 3u);
+    for (uint32_t tid = 0; tid < 3u; ++tid)
+      gk_spec_stage(B, B.scopes, k.x.data(), ki.im.img.data() + (size_t)t * ki.im.stride, k.lo.data(), k.hi.data(), k.stg.data(), tid, 3u);
     k.flags = B.flags;
     k.n = B.n;
     k.t = t;
@@ -266,8 +313,30 @@ extern "C" int gk_spec_host(const GkKParams* p, uint32_t obj, uint32_t* vw, uint
     uint32_t disagree = 0u;
     for (uint32_t o = 0; o < B.n; ++o) disagree += k.walk_wide[o] != (gk_spec_wide(B.scopes, o) ? 1u : 0u);
     std::vector<uint32_t> units, whole;
-    const uint32_t nu = gk_spec_host_plan(B, GK_SPEC_HOST_PLAN_TILE, units, whole);
+    GkSpecHostImage im;
+    const uint32_t nu = gk_spec_host_plan(B, GK_SPEC_HOST_PLAN_TILE, units, whole, im);
     if (getenv("GK_SPEC_TRACE")) {
+      // "[spec offsets] tiles of T: scopes <s>/<parent> ...; rows <the tile's rows of each parent> | ...; stride <S> bytes; runs <R>
+      // bytes; image <I> bytes" (a run: the values gk_spec_stage() copies, padded to 16 bytes)
+      std::string ol = "[spec offsets] tiles of " + std::to_string(GK_SPEC_HOST_PLAN_TILE) + ": scopes";
+      size_t runs = 0;
+      for (uint32_t s = 1; s < GK_SPEC_NS; ++s)
+        if (gk_spec_parent(s) < GK_SPEC_NS) ol += " " + std::to_string(s) + "/" + std::to_string(gk_spec_parent(s));
+      ol += "; rows";
+      for (size_t t = 0; t < whole.size(); ++t) {
+        uint32_t ni = 0u;
+        ol += t ? " |" : "";
+        for (uint32_t s = 1; s < GK_SPEC_NS; ++s) {
+          const uint32_t P = gk_spec_parent(s);
+          if (P >= GK_SPEC_NS) continue;
+          const uint32_t c = im.hi[t * GK_SPEC_NS + P] - im.lo[t * GK_SPEC_NS + P];
+          ol += " " + std::to_string(c);
+          ni += c + 1u;
+        }
+        runs += (ni + 7u) / 8u * 16u;
+      }
+      ol += "; stride " + std::to_string(2u * im.stride) + " bytes; runs " + std::to_string(runs) + " bytes; image " + std::to_string(im.img.size() * 2) + " bytes";
+      fprintf(stderr, "%s\n", ol.c_str());
       std::string line = "[spec plan] tiles of " + std::to_string(GK_SPEC_HOST_PLAN_TILE) + ": " + std::to_string(nu) + " units:";
       for (uint32_t u = 0; u < nu; ++u) line += " " + std::to_string(units[2 * u]) + "+" + std::to_string(units[2 * u + 1]);
       line += "; whole tiles:";
@@ -613,12 +682,12 @@ struct Gen {
   // `rm` = the mask of the children of parent row pj inside the object's rows of scope L, `pb` = the parent row's own bit.  The CSR
   // offsets are monotone, so rm = (rows below the END of pj) & ~(rows below its START), and the start of pj is the end of pj - 1: one
   // load and one mask per turn, carried.  (lo<L> is by definition the offset at lo<P>: the first parent's children start at bit 0.)
-  // q<L> is the tile's slice of the offsets in shared memory, tile-relative (gk_spec_stage).
+  // q<L> is the tile's slice of the offsets in shared memory, tile-relative 16-bit values (gk_spec_stage).
   // Not unrolled: parents have one to three rows here, the unrolled-by-four body the compiler makes is text that never runs.
   std::string range_loop_head(uint32_t L) {
     const uint32_t P = (uint32_t)c.schema.scopes[L].parent;
     const std::string l = std::to_string(L), p = std::to_string(P);
-    return "  {\n  uint32_t lmp = 0u;\n  _Pragma(\"unroll 1\") for (uint32_t pj = 0; pj < n" + p + "; ++pj) {\n    const uint32_t rb = q" + l + "[lo" + p + " + pj + 1u] - lo" + l +
+    return "  {\n  uint32_t lmp = 0u;\n  _Pragma(\"unroll 1\") for (uint32_t pj = 0; pj < n" + p + "; ++pj) {\n    const uint32_t rb = (uint32_t)q" + l + "[lo" + p + " + pj + 1u] - lo" + l +
            ";\n    const uint32_t lm = rb >= 32u ? 0xffffffffu : ((1u << rb) - 1u), rm = lm & ~lmp, pb = 1u << pj;\n    lmp = lm;\n    (void)pb;\n";
   }
 
@@ -982,21 +1051,26 @@ __device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
   for (uint32_t s : nested) out.stage.push_back({parent_of(s), 0u});
   out.stage_hdr = data0;
   out.ngroups = NG;
-  // the per-tile layout: b<s> / c<s> = first row / rows of scope s in the tile, R<g> / Q<s> = region offsets.  Row loop g's region
-  // is ceil(c / 32) + 2 blocks, at least ((b & 31) + c) / 32 + 2: the ceil(((b & 31) + c) / 32) + 1 the copy fills (the tile's rows and
+  out.nested = nested;
+  // the per-tile layout: b<s> / c<s> = first row / rows of scope s in the tile, R<g> = region offsets.  Row loop g's region is
+  // ceil(c / 32) + 2 blocks, at least ((b & 31) + c) / 32 + 2: the ceil(((b & 31) + c) / 32) + 1 the copy fills (the tile's rows and
   // the block after them) and, when (b & 31) + c is a multiple of 32, one more that only the window of an object with no rows there
-  // reads (masked to 0).
-  std::ostringstream lay;
-  lay << "  const uint32_t b0 = GK_SPEC_LD(tlo), c0 = GK_SPEC_LD(thi) - b0;\n  (void)b0; (void)c0;\n";
+  // reads (masked to 0).  Then, at word QA, the tile's run of the offset image (SpecSource::image_stride): nested scope s's offsets
+  // at 16-bit value I<s> of the run, c<parent> + 1 of them; NI values in all, padded to 16 bytes.
+  std::ostringstream tiles, img;
+  tiles << "  const uint32_t b0 = GK_SPEC_LD(tlo), c0 = GK_SPEC_LD(thi) - b0;\n  (void)b0; (void)c0;\n";
   for (uint32_t s : nested)
-    lay << "  const uint32_t b" << s << " = GK_SPEC_LD(tlo + " << s << "), c" << s << " = GK_SPEC_LD(thi + " << s << ") - b" << s << ";\n  (void)c" << s << ";\n";
-  lay << "  uint32_t at = " << data0 << "u;\n";
+    tiles << "  const uint32_t b" << s << " = GK_SPEC_LD(tlo + " << s << "), c" << s << " = GK_SPEC_LD(thi + " << s << ") - b" << s << ";\n  (void)c" << s << ";\n";
+  img << "  uint32_t NI = 0u;\n";
+  for (uint32_t s : nested) img << "  const uint32_t I" << s << " = NI;\n  NI += c" << parent_of(s) << " + 1u;\n";
+  std::ostringstream lay;
+  lay << tiles.str() << "  uint32_t at = " << data0 << "u;\n";
   for (size_t gi = 0; gi < NG; ++gi) {
     const std::string s = std::to_string(group_scope(gi));
     lay << "  const uint32_t R" << gi << " = at;\n";
     if (group_planes(gi)) lay << "  at += ((c" << s << " + 31u) / 32u + 2u) * " << group_planes(gi) << "u;\n";
   }
-  for (uint32_t s : nested) lay << "  const uint32_t Q" << s << " = at;\n  at += c" << parent_of(s) << " + 1u;\n";
+  lay << "  const uint32_t QA = at;\n" << img.str() << "  at += (NI + 7u) / 8u * 4u;\n";
   // X<g> = the word offset of row loop g's planes in the scratch buffer; X<NG> = the buffer's words
   std::ostringstream xbase;
   // (32-bit words: the planes are under one bit per row per export, and a scope's rows fit 32 bits)
@@ -1089,6 +1163,16 @@ __device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
   }
   o << "\n#ifdef GK_SPEC_HOST\n";
   o << "static uint32_t gk_spec_stage_words(const uint32_t* tlo, const uint32_t* thi) {\n" << lay.str() << "  return at;\n}\n";
+  // SpecSource::image_stride and image_fits, over the tiles the host build makes
+  o << "static uint32_t gk_spec_image_stride(const uint32_t* cap) {\n  uint32_t v = 0u;\n";
+  for (uint32_t s : nested) o << "  v += cap[" << parent_of(s) << "] + 1u;\n";
+  o << "  return (v + 7u) / 8u * 8u;\n}\n";
+  o << "static bool gk_spec_image_fits(const uint32_t* cap) {\n  (void)cap;\n  return true";
+  for (uint32_t s : nested) o << " && cap[" << s << "] <= 0xffffu";
+  o << ";\n}\n";
+  o << "// the parent of a nested scope whose offsets are staged, ~0u for any other scope\nstatic uint32_t gk_spec_parent(uint32_t s) {\n  switch (s) {\n";
+  for (uint32_t s : nested) o << "    case " << s << "u: return " << parent_of(s) << "u;\n";
+  o << "    default: return 0xffffffffu;\n  }\n}\n";
   o << "static void gk_spec_tile_rows(const GkScope* scopes, uint32_t* tlo, uint32_t* thi) {\n";
   for (uint32_t s : nested)
     o << "  tlo[" << s << "] = scopes[" << s << "].off[tlo[" << parent_of(s) << "]];\n  thi[" << s << "] = scopes[" << s << "].off[thi[" << parent_of(s) << "]];\n";
@@ -1165,13 +1249,14 @@ __device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
   }
   o << "  }\n";
   o << "}\n#endif\n";
-  // the copy: every 16-byte copy of the tile's plane blocks in flight (cp.async) before the offsets' loads
-  o << "GK_SPEC_FN void gk_spec_stage(const GkBatch& B, const GkScope* scopes, const uint32_t* __restrict__ xs, const uint32_t* tlo, const uint32_t* thi, uint32_t* stg,\n"
-       "                              const uint32_t tid, const uint32_t nthr) {\n  (void)B; (void)xs;\n";
+  // the copy: every 16-byte copy of the tile's plane blocks and of its run of the offset image (`img`) in flight together (cp.async),
+  // one wait.  The header's offsets entries are 16-bit indices from stg.
+  o << "GK_SPEC_FN void gk_spec_stage(const GkBatch& B, const GkScope* scopes, const uint32_t* __restrict__ xs, const uint16_t* __restrict__ img, const uint32_t* tlo,\n"
+       "                              const uint32_t* thi, uint32_t* stg, const uint32_t tid, const uint32_t nthr) {\n  (void)B; (void)xs; (void)img;\n";
   o << lay.str() << xbase.str();
   o << "  if (tid == 0u) {\n";
   for (size_t gi = 0; gi < NG; ++gi) o << "    stg[" << gi << "] = R" << gi << ";\n";
-  for (size_t j = 0; j < nested.size(); ++j) o << "    stg[" << NG + j << "] = Q" << nested[j] << ";\n";
+  for (size_t j = 0; j < nested.size(); ++j) o << "    stg[" << NG + j << "] = 2u * QA + I" << nested[j] << ";\n";
   for (size_t gi = 0; gi < NG; ++gi) o << "    stg[" << NR + gi << "] = b" << group_scope(gi) << " & 31u;\n";
   o << "  }\n";
   for (size_t gi = 0; gi < NG; ++gi) {
@@ -1183,17 +1268,26 @@ __device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
       << "    const uint32_t n = (((b" << s << " & 31u) + c" << s << " + 31u) / 32u + 1u) * " << P / 4 << "u;\n"
       << "    for (uint32_t i = tid; i < n; i += nthr) GK_SPEC_CP16(dst + i, src + i);\n  }\n";
   }
-  // the offsets of sibling scopes are read at the same parent rows: one item stages all of a parent's children (independent loads)
+  if (!nested.empty())
+    o << "  {   // the offsets: the tile's run of the offset image, verbatim\n    const uint4* __restrict__ src = reinterpret_cast<const uint4*>(img);\n"
+      << "    uint4* dst = reinterpret_cast<uint4*>(stg + QA);\n    const uint32_t n = (NI + 7u) / 8u;\n"
+      << "    for (uint32_t i = tid; i < n; i += nthr) GK_SPEC_CP16(dst + i, src + i);\n  }\n";
+  o << "  GK_SPEC_CP_WAIT();\n}\n";
+  // ---- the offset image of one tile (gk_spec_plan_kernel, gk_spec_host_plan): from the batch's CSR offsets, tile-relative, in the
+  // layout gk_spec_stage() copies.  The offsets of sibling scopes are read at the same parent rows: one item writes all of a parent's
+  // children.
+  o << "GK_SPEC_FN void gk_spec_offsets(const GkScope* __restrict__ scopes, const uint32_t* tlo, const uint32_t* thi, uint16_t* img, const uint32_t tid,\n"
+       "                                const uint32_t nthr) {\n  (void)scopes; (void)img; (void)tid; (void)nthr;\n";
+  o << tiles.str() << img.str() << "  (void)NI;\n";
   std::map<uint32_t, std::vector<uint32_t>> children;
   for (uint32_t s : nested) children[parent_of(s)].push_back(s);
   for (auto& ch : children) {
     const uint32_t P = ch.first;
     o << "  for (uint32_t k = tid; k <= c" << P << "; k += nthr) {   // offsets of the children of scope " << P << "\n";
-    for (uint32_t s : ch.second) o << "    const uint32_t x" << s << " = GK_SPEC_LD(scopes[" << s << "].off + b" << P << " + k);\n";
-    for (uint32_t s : ch.second) o << "    stg[Q" << s << " + k] = x" << s << " - b" << s << ";\n";
+    for (uint32_t s : ch.second) o << "    img[I" << s << " + k] = (uint16_t)(GK_SPEC_LD(scopes[" << s << "].off + b" << P << " + k) - b" << s << ");\n";
     o << "  }\n";
   }
-  o << "  GK_SPEC_CP_WAIT();\n}\n";
+  o << "}\n";
   // ---- which objects are WIDE: more rows in some used nested scope than a mask register holds.  The object's row range in scope s,
   // [lo<s>, hi<s>), from its parent's through s's CSR offsets, read by `off(s, row)`.  A scope with more rows than a mask holds
   // counts as EMPTY from there on and raises `big`: no branch.  gk_spec_object() reads the tile's staged offsets, gk_spec_wide()
@@ -1223,8 +1317,8 @@ __device__ __forceinline__ uint32_t gk_tr32(uint32_t x, uint32_t lane) {
   o << "  bool big = false;\n";
   for (size_t j = 0; j < nested.size(); ++j) {
     const uint32_t s = nested[j];
-    o << "  const uint32_t* __restrict__ q" << s << " = stg + stg[" << NG + j << "];\n";
-    scope_extent(s, [&](const std::string& row) { return "q" + std::to_string(s) + "[" + row + "]"; });
+    o << "  const uint16_t* __restrict__ q" << s << " = reinterpret_cast<const uint16_t*>(stg) + stg[" << NG + j << "];\n";
+    scope_extent(s, [&](const std::string& row) { return "(uint32_t)q" + std::to_string(s) + "[" + row + "]"; });
     o << "  const uint32_t f" << s << " = n" << s << " >= 32u ? 0xffffffffu : ((1u << n" << s << ") - 1u);\n  (void)hi" << s << "; (void)f" << s << ";\n";
   }
   // the object's rows of scope s start at bit e<g> of row loop g's staged planes: plane k's 32-bit window there, bit j = row j of the

@@ -29,12 +29,29 @@ struct SpecSource {
   // row loops' export planes, in row-loop order; the rest the nested scopes' offsets)
   struct StageRegion {
     // a row loop: `planes` export planes (its exports rounded up to 4), one word per plane per block of 32 rows of `scope`; a
-    // nested scope's offsets: one word per row of `scope` (its parent) + 1 (planes = 0)
+    // nested scope's offsets: one 16-bit value per row of `scope` (its parent) + 1 (planes = 0)
     uint32_t scope, planes;
   };
   std::vector<StageRegion> stage;
   uint32_t stage_hdr = 0;
   uint32_t ngroups = 0;
+  std::vector<uint32_t> nested;   // the used nested scopes, whose offsets are staged: stage[ngroups + j] is nested[j]'s
+  // The offset image (gk_spec_plan_kernel writes it once per batch and text, gk_spec_stage copies a tile's run verbatim): per tile,
+  // the offsets regions of the staging area back to back, every nested scope's tile-relative CSR offsets as 16-bit values, the run
+  // padded to 16 bytes; tile t's run at t * image_stride(cap) values.  The stride bounds every tile's run from the largest tile's
+  // rows per scope (cap), as stage_bytes() bounds the staging area.
+  uint32_t image_stride(const std::vector<uint32_t>& cap) const {
+    uint64_t v = 0;
+    for (size_t i = ngroups; i < stage.size(); ++i) v += (uint64_t)(stage[i].scope < cap.size() ? cap[stage[i].scope] : 0u) + 1u;
+    return (uint32_t)((v + 7) / 8 * 8);
+  }
+  // A tile-relative offset of scope s is at most the tile's rows of s: the image holds them when no tile has more than 65535 rows
+  // in a nested scope.  A batch with such a tile (only objects far too wide for the mask registers make one) is interpreted.
+  bool image_fits(const std::vector<uint32_t>& cap) const {
+    for (uint32_t s : nested)
+      if (s < cap.size() && cap[s] > 0xffffu) return false;
+    return true;
+  }
   // per scope with atoms: what a row evaluates (atoms, row-local gates) and what it exports (by read form; on scope 0 the mask-form
   // exports include the match and error bits of the spec.match blocks), in `words` words per row
   struct Fold {
@@ -55,14 +72,12 @@ struct SpecSource {
     return t;
   }
   // bytes of the staging area for a batch whose largest tile has cap[s] rows in scope s: a tile's rows of a scope start anywhere in
-  // a block of 32, so they span at most ceil(cap / 32) + 1 blocks, and the region holds one more (gk_spec_stage)
+  // a block of 32, so they span at most ceil(cap / 32) + 1 blocks, and the region holds one more (gk_spec_stage); then one run of
+  // the offset image.  (Every region is a multiple of 16 bytes, so the offsets start 16-byte aligned.)
   size_t stage_bytes(const std::vector<uint32_t>& cap) const {
     size_t w = stage_hdr;
-    for (size_t i = 0; i < stage.size(); ++i) {
-      const size_t rows = stage[i].scope < cap.size() ? cap[stage[i].scope] : 0u;
-      w += i < ngroups ? ((rows + 31) / 32 + 2) * stage[i].planes : rows + 1;
-    }
-    return w * 4;
+    for (size_t i = 0; i < ngroups; ++i) w += (((size_t)(stage[i].scope < cap.size() ? cap[stage[i].scope] : 0u) + 31) / 32 + 2) * stage[i].planes;
+    return w * 4 + (size_t)image_stride(cap) * 2;
   }
   // bytes of the export planes (gk_spec_rows_kernel -> gk_spec_kernel) of a batch with rows[s] rows in scope s (rows[0] = objects):
   // per row loop, `planes` words per block of 32 rows and one guard block (a window's high word past the last block)

@@ -98,7 +98,7 @@ def static_report(cubin_path: str, cu_path: str):
                 else:
                     region["rows: loads, atoms, control"] += 1
             elif stage <= cur < start:
-                region["tile: copy of the exports and offsets"] += 1
+                region["tile: copy of the exports and offsets" if kern == "tile" else kern + ": offset image and wide test"] += 1
             elif cur < start:
                 region[kern + ": spec.match (written-out blocks / vm_core.h)"] += 1
             elif cur < end:
