@@ -101,12 +101,19 @@ class Backend {
   virtual void* ingest(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status) = 0;
   // Keeping a page's source for a refresh after a constraint change (gk_batch_refresh, GK_F_KEEP_SOURCE).  ingest_keep() is ingest()
   // that also hands the caller the page's source in *keep; reextract() builds a new batch from it for the program of rq.c without
-  // reading the caller's page (rq.blob / rq.ooff are not read); release_source() frees it.  The CUDA backend keeps the page's device
+  // reading the caller's page (rq.blob / rq.ooff are not read) -- `status` (may be null) receives its objects' GK_ING_* codes;
+  // release_source() frees it.  The CUDA backend keeps the page's device
   // JSON, offsets and token tape and re-runs only the extraction passes.  These defaults, for a backend whose pages do not stay on a
   // device (the test-only host emulation), keep a host copy of the page and ingest it again.
   virtual void* ingest_keep(const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status, void** keep);
-  virtual void* reextract(void* source, const IngestReq& rq, IngestStats* st);
+  virtual void* reextract(void* source, const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status);
   virtual void release_source(void* source);
+  // A new page source for gk_batch_patch: objects `keep` of `source` (ascending, each at most once), then the n_add documents of
+  // blob / ooff (object k at blob[ooff[k], ooff[k+1])), as a source kept by ingest_keep() of that page would be.  `source` stays
+  // as it was; the caller's page is not read after the call.  The CUDA backend moves the staying objects' JSON and token tape on the
+  // device and copies and tokenises only the added documents; this default concatenates host copies.
+  virtual void* patch_source(void* source, const std::vector<uint32_t>& keep, const uint8_t* blob, const unsigned long long* ooff, size_t n_add,
+                             IngestStats* st);
   // The JSON of objects `idx` of a kept page source, back to back into `bytes`, object k at [off[k], off[k+1]) (an expanded batch's
   // refresh, which does not read the caller's page).  The CUDA backend gathers them from the page's device copy.
   virtual void source_bytes(void* source, const std::vector<uint32_t>& idx, std::string& bytes, std::vector<uint64_t>& off);
@@ -170,17 +177,36 @@ inline void* Backend::ingest_keep(const IngestReq& rq, IngestStats* st, std::vec
   *keep = src.release();
   return b;
 }
-inline void* Backend::reextract(void* source, const IngestReq& rq, IngestStats* st) {
+inline void* Backend::reextract(void* source, const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status) {
   auto* src = static_cast<HostPageCopy*>(source);
   if (!src || src->ooff.size() != rq.n + 1) throw BackendError{"device ingest: the kept source is of another page"};
   IngestReq r = rq;
   r.blob = src->blob.data();
   r.ooff = src->ooff.data();
   r.lut_fill = [&rq, src](const GkMiss* m, size_t k, std::vector<GkLutVal>& out) { rq.lut_fill_from(src->blob.data(), m, k, out); };
-  std::vector<uint32_t> status;
-  return ingest(r, st, &status);
+  std::vector<uint32_t> own;
+  return ingest(r, st, status ? status : &own);
 }
 inline void Backend::release_source(void* source) { delete static_cast<HostPageCopy*>(source); }
+inline void* Backend::patch_source(void* source, const std::vector<uint32_t>& keep, const uint8_t* blob, const unsigned long long* ooff, size_t n_add,
+                                   IngestStats* st) {
+  auto* old = static_cast<HostPageCopy*>(source);
+  if (!old) throw BackendError{"kept source: none"};
+  auto src = std::make_unique<HostPageCopy>();
+  src->ooff.assign(1, 0);
+  for (uint32_t i : keep) {
+    if ((size_t)i + 1 >= old->ooff.size()) throw BackendError{"kept source: object index out of range"};
+    src->blob.insert(src->blob.end(), old->blob.begin() + old->ooff[i], old->blob.begin() + old->ooff[i + 1]);
+    src->ooff.push_back(src->blob.size());
+  }
+  for (size_t k = 0; k < n_add; ++k) {
+    src->blob.insert(src->blob.end(), blob + ooff[k], blob + ooff[k + 1]);
+    src->ooff.push_back(src->blob.size());
+  }
+  src->blob.resize(src->blob.size() + 16, 0);
+  if (st) *st = IngestStats{};
+  return src.release();
+}
 inline void Backend::source_bytes(void* source, const std::vector<uint32_t>& idx, std::string& bytes, std::vector<uint64_t>& off) {
   auto* src = static_cast<HostPageCopy*>(source);
   bytes.clear();

@@ -155,6 +155,8 @@ struct gk_batch {
   std::vector<std::string> source_errors;
   std::shared_ptr<Expanded> ex;        // GK_F_EXPAND: the page's resultants (null: a batch uploaded without the flag)
   ObjIn obj_in(size_t i) const;
+  // a page of plain objects of one source (gk_batch_upload_blob): `blob`, or -- once patched (gk_batch_patch) -- `objs`, one span each
+  bool plain_page() const { return blob || source; }
 };
 
 namespace {
@@ -494,6 +496,17 @@ bool device_ingest(const Compiled& c, size_t n) {
   return c.device_ingest && !host_only && n != 0 && !getenv("GK_NO_DEVICE_INGEST_RUNTIME");   // (the runtime switch is for A/B tests)
 }
 
+// the review-level error of an object the device ingest rejected (`status`: its GK_ING_* code), worded by the host parser (bad JSON,
+// not an object, kind missing)
+std::string ingest_error(gk_engine* e, uint32_t status, const ObjIn& in) {
+  std::string err;
+  VP doc = e->eng->review_doc(in, nullptr, nullptr, nullptr, &err);
+  if (doc && status != GK_ING_NULL) err = "device ingest refused the object (status " + std::to_string(status) + "): JSON nesting deeper than " +
+                                          std::to_string(GK_TAPE_MAX_DEPTH) + " levels or a token longer than 128 MiB";
+  if (!doc && err.empty()) err = "invalid request object";
+  return err;
+}
+
 // a blob of plain objects: flattened by the ingest kernels on the device when the compiled snapshot allows it
 std::unique_ptr<gk_batch> upload_blob(gk_engine* e, const std::shared_ptr<const Compiled>& c, const char* buf, const uint64_t* off, size_t n, uint8_t source,
                                       uint32_t flags, gk_result* stats) {
@@ -513,17 +526,11 @@ std::unique_ptr<gk_batch> upload_blob(gk_engine* e, const std::shared_ptr<const 
     for (size_t i = 0; i < n; ++i)
       if (status[i] != GK_ING_OK) {
         if (errors.empty()) errors.assign(n, std::string());   // (left empty when every object is fine)
-        // the rare rejected object: the host parser words the review-level error (bad JSON, not an object, kind missing)
         ObjIn in;
         in.json = buf + off[i];
         in.len = (size_t)(off[i + 1] - off[i]);
         in.source = source;
-        std::string err;
-        VP doc = e->eng->review_doc(in, nullptr, nullptr, nullptr, &err);
-        if (doc && status[i] != GK_ING_NULL) err = "device ingest refused the object (status " + std::to_string(status[i]) + "): JSON nesting deeper than " +
-                                                 std::to_string(GK_TAPE_MAX_DEPTH) + " levels or a token longer than 128 MiB";
-        if (!doc && err.empty()) err = "invalid request object";
-        errors[i] = err;
+        errors[i] = ingest_error(e, status[i], in);
       }
     b = make_batch(e, c, std::move(dev), (uint32_t)n, flags, errors, std::move(rq.excluded), ist, (now_ms() - t0) - ist.h2d_ms, stats);
     if (source_kept) {
@@ -543,8 +550,9 @@ std::unique_ptr<gk_batch> refresh_from_source(gk_engine* e, const std::shared_pt
   double t0 = now_ms();
   IngestReq rq = e->eng->ingest_request(c, nullptr, nullptr, old.n, old.blob_source, process_of(old.flags));
   IngestStats ist;
-  BackendHandle dev = device_batch(e, e->be->reextract(old.source.get(), rq, &ist));
+  BackendHandle dev = device_batch(e, e->be->reextract(old.source.get(), rq, &ist, nullptr));
   auto b = make_batch(e, c, std::move(dev), old.n, old.flags, old.source_errors, std::move(rq.excluded), ist, (now_ms() - t0) - ist.h2d_ms, stats);
+  b->objs = old.objs;
   b->blob = old.blob;
   b->blob_off = old.blob_off;
   b->blob_source = old.blob_source;
@@ -687,7 +695,7 @@ void expand_batch(gk_engine* e, const std::shared_ptr<const Compiled>& c, gk_bat
   const size_t m = x.children.size();
   const uint32_t rflags = b.flags & ~(uint32_t)(GK_F_KEEP_SOURCE | GK_F_EXPAND);
   if (m) {
-    if (b.blob) {   // blob parents (no Namespace objects): the resultants as one page, for the device ingest
+    if (b.plain_page()) {   // blob parents (no Namespace objects): the resultants as one page, for the device ingest
       ex->off.assign(1, 0);
       for (auto& ch : x.children) {
         ex->blob += ch.json;
@@ -1041,15 +1049,16 @@ int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err
     }
     ProgramLease lease(e, *c);
     std::unique_ptr<gk_batch> nb;
-    const bool from_source = b->blob && b->source && device_ingest(*c, b->n);
-    if (!b->blob) nb = upload_batch(e, c, b->objs.data(), b->objs.size(), b->flags, stats);
-    else if (from_source) nb = refresh_from_source(e, c, *b, stats);
+    const bool from_source = b->source && device_ingest(*c, b->n);
+    if (from_source) nb = refresh_from_source(e, c, *b, stats);
+    else if (!b->blob) nb = upload_batch(e, c, b->objs.data(), b->objs.size(), b->flags, stats);
     else nb = upload_blob(e, c, b->blob, b->blob_off, b->n, b->blob_source, b->flags, stats);
     // the new columns replace the old ones; a kept source stays with the batch (a batch that had none may have gained one)
     if (!nb->source) {
       nb->source = std::move(b->source);
       nb->source_errors = std::move(b->source_errors);
     }
+    nb->blob_source = b->blob_source;   // (a patched page flattened on the host: its objects are review objects of that source)
     if (b->flags & GK_F_EXPAND) {   // (expanded again whatever changed: the resultants' columns follow the constraint set too)
       expand_batch(e, c, *nb, xv, from_source);
       if (stats) stats->alg_bytes = nb->alg_bytes;
@@ -1058,6 +1067,90 @@ int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err
     rebuilt = true;
   });
   return rc == GK_OK && rebuilt ? 1 : rc;
+}
+
+int gk_batch_patch(gk_engine_t* e, gk_batch_t* b, const uint32_t* drop, size_t n_drop, const char* buf, const uint64_t* offsets, size_t n_add,
+                   gk_result* stats, char** err) {
+  if (!e || !b || (!drop && n_drop) || ((!buf || !offsets) && n_add)) return GK_ERR_INVALID;
+  if (stats) memset(stats, 0, sizeof *stats);
+  auto invalid = [err](const std::string& why) {
+    if (err) *err = dup_str(why);
+    return GK_ERR_INVALID;
+  };
+  if (!b->source)
+    return invalid("the batch keeps no device source to patch: only a gk_batch_upload_blob batch uploaded with GK_F_KEEP_SOURCE while its constraint "
+                   "set was flattened on the device keeps one; upload the page again");
+  std::vector<uint8_t> dropped(b->n, 0);
+  for (size_t k = 0; k < n_drop; ++k) {
+    if (drop[k] >= b->n) return invalid("drop index " + std::to_string(drop[k]) + " is out of range: the batch holds " + std::to_string(b->n) + " objects");
+    if (dropped[drop[k]]++) return invalid("drop index " + std::to_string(drop[k]) + " is given twice");
+  }
+  if ((uint64_t)b->n - n_drop + n_add > 0x7fffff00ull) return invalid("a patched batch would hold more than 2^31 objects");
+  int refused = 0;
+  const int rc = guard(err, [&]() {
+    const uint64_t xv = e->eng->expansion_version();
+    auto c = e->eng->compiled();
+    if (!device_ingest(*c, 1)) {   // (a fresh upload would flatten the page on the host and keep no device source)
+      refused = invalid("the constraint set is flattened on the host (" + (c->host_ingest_reason.empty() ? std::string("device ingest turned off") : c->host_ingest_reason) +
+                        "): a patch splices the page on the device only; upload the page again");
+      return;
+    }
+    ProgramLease lease(e, *c);
+    const double t0 = now_ms();
+    std::vector<uint32_t> keep;
+    keep.reserve(b->n - n_drop);
+    for (uint32_t i = 0; i < b->n; ++i)
+      if (!dropped[i]) keep.push_back(i);
+    const uint32_t nk = (uint32_t)keep.size(), n = nk + (uint32_t)n_add;
+    IngestStats pst;
+    BackendHandle src = kept_source(e, e->be->patch_source(b->source.get(), keep, reinterpret_cast<const uint8_t*>(buf),
+                                                           reinterpret_cast<const unsigned long long*>(offsets), n_add, &pst));
+    // the objects as the host reads them (messages, audit, expansion): the staying ones where they were given, the added ones in buf
+    std::vector<gk_obj> objs(n);
+    for (uint32_t j = 0; j < n; ++j) {
+      gk_obj& o = objs[j];
+      memset(&o, 0, sizeof o);
+      if (j < nk) {
+        const ObjIn in = b->obj_in(keep[j]);
+        o.json = in.json;
+        o.len = in.len;
+      } else {
+        o.json = buf + offsets[j - nk];
+        o.len = (size_t)(offsets[j - nk + 1] - offsets[j - nk]);
+      }
+      o.source = b->blob_source;
+    }
+    std::unique_ptr<gk_batch> nb;
+    std::vector<std::string> errors;
+    if (n) {
+      IngestReq rq = e->eng->ingest_request(c, nullptr, nullptr, n, b->blob_source, process_of(b->flags));
+      IngestStats ist;
+      std::vector<uint32_t> status;
+      BackendHandle dev = device_batch(e, e->be->reextract(src.get(), rq, &ist, &status));
+      for (uint32_t j = 0; j < n; ++j)
+        if (status[j] != GK_ING_OK) {
+          if (errors.empty()) errors.assign(n, std::string());
+          errors[j] = j < nk && !b->source_errors.empty() ? b->source_errors[keep[j]] : ingest_error(e, status[j], to_in(objs[j]));
+        }
+      ist.h2d_ms += pst.h2d_ms;
+      ist.h2d_bytes += pst.h2d_bytes;
+      nb = make_batch(e, c, std::move(dev), n, b->flags, errors, std::move(rq.excluded), ist, (now_ms() - t0) - ist.h2d_ms, stats);
+      if (stats) stats->kernel_ms = pst.h2d_ms + ist.extract_ms;
+    } else {
+      nb = upload_batch(e, c, nullptr, 0, b->flags, stats);   // (as gk_batch_upload_blob of an empty page)
+    }
+    nb->objs = std::move(objs);
+    nb->blob_source = b->blob_source;
+    nb->source = std::move(src);
+    nb->source_errors = std::move(errors);
+    if (b->flags & GK_F_EXPAND) {
+      expand_batch(e, c, *nb, xv, true);
+      if (stats) stats->alg_bytes = nb->alg_bytes;
+    }
+    std::swap(*b, *nb);   // (the old columns and source are released with nb)
+  });
+  if (rc != GK_OK) return rc;
+  return refused ? refused : (int)b->n;
 }
 
 int gk_set_excluded_namespaces(gk_engine_t* e, const char* process, const char* const* patterns, size_t n, char** err) {

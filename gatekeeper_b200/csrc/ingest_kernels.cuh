@@ -9,6 +9,8 @@
 //   gk_scan_*             exclusive prefix sums (counts -> CSR offsets), three small kernels for any length
 //   gk_fill_kernel        the host's answers to the miss list -> table slots
 //   gk_gather_kernel      the argument bytes of the miss list, when the host's copy of the page is not at hand (a kept source)
+//   gk_keep_len_kernel    gk_batch_patch: byte lengths of a kept page's staying objects (scanned into their new offsets)
+//   gk_splice_kernel      gk_batch_patch: one warp per staying object moves its JSON, tape, tape length and status to the new page
 //   gk_tiles_kernel       first row of every scope for every evaluation tile + the largest tile of each scope
 // Level-synchronous: every kernel after the tokeniser runs ONE step for all rows of ONE scope, so the threads of a warp follow
 // the same path (the per-object walk of the whole scope tree it replaces ran at 1.7 active threads per warp instruction).
@@ -187,6 +189,54 @@ __global__ void gk_gather_kernel(uint8_t* dst, const uint8_t* blob, const unsign
   for (uint32_t k = blockIdx.x; k < nspans; k += gridDim.x) {
     const unsigned long long src = spans[3 * k], to = spans[3 * k + 1], len = spans[3 * k + 2];
     for (unsigned long long i = threadIdx.x; i < len; i += blockDim.x) dst[to + i] = blob[src + i];
+  }
+}
+
+// ---- gk_batch_patch: a kept page's staying objects moved into a new page
+// len[j] = byte length of staying object keep[j] of the old page; len[n_keep] = 0, so that an exclusive scan over n_keep + 1
+// entries gives the staying objects' offsets in the new page and, last, their total
+__global__ void gk_keep_len_kernel(const unsigned long long* ooff, const uint32_t* keep, uint32_t n_keep, unsigned long long* len) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n_keep) len[j] = ooff[keep[j] + 1] - ooff[keep[j]];
+  else if (j == n_keep) len[j] = 0;
+}
+
+// one warp copies len bytes in words of W, with byte copies before the first aligned destination word and after the last one
+// (src and dst agree modulo sizeof(W))
+template <class W>
+__device__ void gk_warp_copy_words(uint8_t* dst, const uint8_t* src, unsigned long long len, uint32_t lane) {
+  const unsigned long long head = min((unsigned long long)((sizeof(W) - (reinterpret_cast<size_t>(dst) & (sizeof(W) - 1))) & (sizeof(W) - 1)), len);
+  for (unsigned long long k = lane; k < head; k += 32) dst[k] = src[k];
+  const unsigned long long words = (len - head) / sizeof(W);
+  W* d = reinterpret_cast<W*>(dst + head);
+  const W* s = reinterpret_cast<const W*>(src + head);
+  for (unsigned long long k = lane; k < words; k += 32) d[k] = s[k];
+  for (unsigned long long k = head + words * sizeof(W) + lane; k < len; k += 32) dst[k] = src[k];
+}
+__device__ void gk_warp_copy(uint8_t* dst, const uint8_t* src, unsigned long long len, uint32_t lane) {
+  const uint32_t mis = (uint32_t)((reinterpret_cast<size_t>(dst) ^ reinterpret_cast<size_t>(src)) & 15u);
+  if (mis == 0u) gk_warp_copy_words<uint4>(dst, src, len, lane);
+  else if ((mis & 7u) == 0u) gk_warp_copy_words<unsigned long long>(dst, src, len, lane);
+  else if ((mis & 3u) == 0u) gk_warp_copy_words<uint32_t>(dst, src, len, lane);
+  else gk_warp_copy_words<uint8_t>(dst, src, len, lane);
+}
+
+// One warp per staying object j (= old object keep[j]): its JSON bytes, its tape entries and its tape length and status word.
+// Tape entries hold positions relative to the object's own first byte (gk_tape_obj tokenises in.blob + ooff[i] as a text of its
+// own), so they move as they are; only where the tape starts, gk_tape_off of the object's offset, changes.  `blob`: to.blob, writable.
+__global__ void __launch_bounds__(256) gk_splice_kernel(const GkIngestIn to, uint8_t* blob, const GkIngestIn from, const uint32_t* keep, uint32_t n_keep) {
+  const uint32_t lane = threadIdx.x & 31u, warps = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n_keep; j += warps) {
+    const uint32_t i = keep[j];
+    const unsigned long long a = from.ooff[i];
+    gk_warp_copy(blob + to.ooff[j], from.blob + a, from.ooff[i + 1] - a, lane);
+    const uint32_t nt = from.ntape[i];
+    gk_warp_copy(reinterpret_cast<uint8_t*>(to.tape + gk_tape_off(to.ooff, j)), reinterpret_cast<const uint8_t*>(from.tape + gk_tape_off(from.ooff, i)),
+                 (unsigned long long)nt * 8u, lane);
+    if (lane == 0) {
+      to.ntape[j] = nt;
+      to.status[j] = from.status[i];
+    }
   }
 }
 

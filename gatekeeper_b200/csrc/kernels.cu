@@ -1198,13 +1198,86 @@ class CudaBackend : public Backend {
     return db;
   }
 
-  void* reextract(void* source, const IngestReq& rq, IngestStats* st) override {
+  void* reextract(void* source, const IngestReq& rq, IngestStats* st, std::vector<uint32_t>* status) override {
     std::lock_guard<std::mutex> l(ingest_mu_);
     CK(cudaSetDevice(device_));
     auto* ks = static_cast<KeptSource*>(source);
     if (!ks || ks->in.n != rq.n) throw BackendError{"device ingest: the kept source is of another page"};
     if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[launch] extraction of %u objects from the kept source: no copy, no tokeniser\n", ks->in.n);
-    return extract(rq, [ks]() { return ks->in; }, ks->bytes, false, st, nullptr);
+    return extract(rq, [ks]() { return ks->in; }, ks->bytes, false, st, status);
+  }
+
+  // A new page from a kept one (gk_batch_patch): the staying objects' offsets by one scan over their lengths, their JSON, tape,
+  // tape lengths and status words moved by gk_splice_kernel, then the added documents copied and tokenised into the tail by the
+  // front buffer's code.  Nothing of the old page is changed; it is freed by its owner.
+  void* patch_source(void* source, const std::vector<uint32_t>& keep, const uint8_t* blob, const unsigned long long* ooff, size_t n_add,
+                     IngestStats* st) override {
+    std::lock_guard<std::mutex> l(ingest_mu_);
+    CK(cudaSetDevice(device_));
+    auto* old = static_cast<KeptSource*>(source);
+    if (!old) throw BackendError{"kept source: none"};
+    const uint32_t nk = (uint32_t)keep.size();
+    if ((uint64_t)nk + n_add > 0x7fffff00ull) throw BackendError{"device ingest: more than 2^31 objects in one batch"};
+    const uint32_t n = nk + (uint32_t)n_add;
+    const unsigned long long add_bytes = n_add ? ooff[n_add] - ooff[0] : 0ull;
+    Event e0, e1;
+    CK(cudaEventRecord(e0, stream_));
+    // ---- the staying objects' new offsets, and their bytes' total
+    Temps temps(this);
+    auto* d_keep = temps.take<uint32_t>((size_t)nk * 4 + 4);
+    auto* d_len = temps.take<unsigned long long>(((size_t)nk + 1) * 8);
+    auto* d_off = temps.take<unsigned long long>(((size_t)nk + 1) * 8);
+    if (nk) CK(cudaMemcpyAsync(d_keep, keep.data(), (size_t)nk * 4, cudaMemcpyHostToDevice, stream_));
+    gk_keep_len_kernel<<<(nk + 1 + 255) / 256, 256, 0, stream_>>>(old->in.ooff, d_keep, nk, d_len);
+    size_t scan_bytes = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_len, d_off, (int64_t)nk + 1, stream_));
+    CK(cub::DeviceScan::ExclusiveSum(temps.take(scan_bytes), scan_bytes, d_len, d_off, (int64_t)nk + 1, stream_));
+    launches_ += 2;
+    unsigned long long kept_bytes = 0;
+    CK(cudaMemcpyAsync(&kept_bytes, d_off + nk, 8, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    CK(cudaGetLastError());
+    // ---- the new page: staying objects first, then the added ones
+    const unsigned long long B = kept_bytes + add_bytes;
+    const PageLayout lay(B, n);
+    auto ks = std::make_unique<KeptSource>();
+    CK(cudaMalloc(&ks->buf, lay.total));
+    ks->in = lay.at(ks->buf);
+    ks->bytes = B;
+    uint8_t* d_ooff = ks->buf + lay.o_ooff;
+    CK(cudaMemcpyAsync(d_ooff, d_off, ((size_t)nk + 1) * 8, cudaMemcpyDeviceToDevice, stream_));
+    if (n_add) {
+      std::vector<unsigned long long> tail(n_add);
+      for (size_t k = 0; k < n_add; ++k) tail[k] = kept_bytes + (ooff[k + 1] - ooff[0]);
+      CK(cudaMemcpyAsync(d_ooff + ((size_t)nk + 1) * 8, tail.data(), n_add * 8, cudaMemcpyHostToDevice, stream_));
+    }
+    CK(cudaMemsetAsync(ks->buf + lay.o_blob + B, 0, 16, stream_));
+    if (nk) {
+      gk_splice_kernel<<<std::min<uint32_t>((nk + 7) / 8, (uint32_t)sms_ * 16), 256, 0, stream_>>>(ks->in, ks->buf + lay.o_blob, old->in, d_keep, nk);
+      ++launches_;
+    }
+    if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[launch] gk_splice_kernel over %u staying objects, %llu bytes\n", nk, kept_bytes);
+    Event spliced;
+    CK(cudaEventRecord(spliced, stream_));
+    {
+      std::lock_guard<std::mutex> fl(front_mu_);
+      CK(cudaStreamWaitEvent(copy_stream_, spliced, 0));   // (the tail's offsets are in place)
+      copy_and_tokenise(ks->in, ks->buf + lay.o_blob + kept_bytes, nk, blob, ooff, (uint32_t)n_add);
+      cudaEvent_t done = chunk_event(0);
+      CK(cudaEventRecord(done, front_stream_));
+      CK(cudaStreamWaitEvent(stream_, done, 0));
+    }
+    CK(cudaEventRecord(e1, stream_));
+    CK(cudaStreamSynchronize(stream_));   // (the temporaries are freed on stream_ and the caller's page may change once this returns)
+    CK(cudaGetLastError());
+    if (st) {
+      float ms = 0;
+      cudaEventElapsedTime(&ms, e0, e1);
+      st->h2d_ms = ms;   // splice, copy and tokeniser
+      st->h2d_bytes = add_bytes + (n_add + (size_t)nk) * 8;
+      st->launches = launches_;
+    }
+    return ks.release();
   }
 
   void source_bytes(void* source, const std::vector<uint32_t>& idx, std::string& bytes, std::vector<uint64_t>& off) override {
@@ -1865,29 +1938,52 @@ class CudaBackend : public Backend {
     bool pending = false;       // prefetched, not yet consumed
     cudaEvent_t done = nullptr; // copy + tokenise finished
   };
+  // The layout of a page's front buffer for B bytes of JSON and n objects: the JSON (16 bytes over, for the tokeniser's word
+  // reads), the offsets, the tape (object i's at gk_tape_off), the tape lengths and the status words.  bytes(): the whole buffer.
+  struct PageLayout {
+    size_t o_blob, o_ooff, o_tape, o_ntape, o_status, total;
+    uint32_t n;
+    PageLayout(unsigned long long B, uint32_t nn) : n(nn) {
+      Carver sc;
+      o_blob = sc.take((size_t)B + 16), o_ooff = sc.take(((size_t)n + 1) * 8), o_tape = sc.take(((size_t)(B / 2) + 4ull * n + 64) * 8),
+      o_ntape = sc.take((size_t)n * 4), o_status = sc.take((size_t)n * 4);
+      total = gk_align(sc.off);
+    }
+    GkIngestIn at(uint8_t* d) const {
+      GkIngestIn in;
+      memset(&in, 0, sizeof in);
+      in.blob = d + o_blob;
+      in.ooff = reinterpret_cast<const unsigned long long*>(d + o_ooff);
+      in.tape = reinterpret_cast<unsigned long long*>(d + o_tape);
+      in.ntape = reinterpret_cast<uint32_t*>(d + o_ntape);
+      in.status = reinterpret_cast<uint32_t*>(d + o_status);
+      in.n = n;
+      return in;
+    }
+  };
+
   Front& start_front(const uint8_t* blob, const unsigned long long* ooff, size_t nn) {   // (front_mu_ held)
     Front& f = fronts_[next_front_];
     next_front_ ^= 1;
     const uint32_t n = (uint32_t)nn;
-    const unsigned long long B = ooff[n];
-    Carver sc;
-    const size_t o_blob = sc.take((size_t)B + 16), o_ooff = sc.take(((size_t)n + 1) * 8), o_tape = sc.take(((size_t)(B / 2) + 4ull * n + 64) * 8),
-                 o_ntape = sc.take((size_t)n * 4), o_status = sc.take((size_t)n * 4);
+    const PageLayout lay(ooff[n], n);
     if (!f.done) CK(cudaEventCreateWithFlags(&f.done, cudaEventDisableTiming));
     // the buffer may still be read by the kernels of the page that used it last: they ran on the main stream
     CK(cudaStreamSynchronize(stream_));
-    uint8_t* d = f.buf.need(gk_align(sc.off));
-    memset(&f.in, 0, sizeof f.in);
-    f.in.blob = d + o_blob;
-    f.in.ooff = reinterpret_cast<const unsigned long long*>(d + o_ooff);
-    f.in.tape = reinterpret_cast<unsigned long long*>(d + o_tape);
-    f.in.ntape = reinterpret_cast<uint32_t*>(d + o_ntape);
-    f.in.status = reinterpret_cast<uint32_t*>(d + o_status);
-    f.in.n = n;
+    uint8_t* d = f.buf.need(lay.total);
+    f.in = lay.at(d);
     f.host_blob = blob;
     f.n = nn;
-    // H2D of the raw JSON in chunks on the copy stream; the tokeniser of a chunk starts as soon as its bytes have landed
-    CK(cudaMemcpyAsync(d + o_ooff, ooff, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, copy_stream_));
+    CK(cudaMemcpyAsync(d + lay.o_ooff, ooff, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, copy_stream_));
+    copy_and_tokenise(f.in, d + lay.o_blob + ooff[0], 0, blob, ooff, n);
+    CK(cudaEventRecord(f.done, front_stream_));
+    f.pending = true;
+    return f;
+  }
+  // Objects [0, cnt) of a host page (JSON at blob + ooff[k]) become objects first .. first + cnt - 1 of the device page `in`, their
+  // bytes at dst + (ooff[k] - ooff[0]), where in.ooff already places them: the JSON goes over in chunks on the copy stream, and the
+  // tokeniser of a chunk starts on the front stream as soon as its bytes have landed.  (front_mu_ held)
+  void copy_and_tokenise(const GkIngestIn& in, uint8_t* dst, uint32_t first, const uint8_t* blob, const unsigned long long* ooff, uint32_t cnt) {
     // Chunk size: a tokeniser launch of a 32 MB chunk (50k Pods) fills a small share of the warp slots and takes about the same
     // time whatever its size (one thread walks one object); bigger chunks mean fewer, fuller launches at the price of a later
     // start, much smaller ones multiply the page time.  GK_INGEST_CHUNK_MB overrides.
@@ -1896,27 +1992,25 @@ class CudaBackend : public Backend {
       if (const char* ev = getenv("GK_INGEST_CHUNK_MB")) mb = (size_t)std::max(1, atoi(ev));
       return mb << 20;
     }();
-    uint32_t first = 0;
-    while (first < n) {
-      uint32_t last = first;
-      const unsigned long long lo = ooff[first];
-      while (last < n && ooff[last + 1] - lo <= kChunk) ++last;
-      if (last == first) ++last;   // one object larger than a chunk
+    uint32_t k = 0;
+    while (k < cnt) {
+      uint32_t last = k;
+      const unsigned long long lo = ooff[k];
+      while (last < cnt && ooff[last + 1] - lo <= kChunk) ++last;
+      if (last == k) ++last;   // one object larger than a chunk
       const unsigned long long hi = ooff[last];
-      CK(cudaMemcpyAsync(d + o_blob + lo, blob + lo, (size_t)(hi - lo), cudaMemcpyHostToDevice, copy_stream_));
-      cudaEvent_t ev = chunk_event(first);
+      CK(cudaMemcpyAsync(dst + (lo - ooff[0]), blob + lo, (size_t)(hi - lo), cudaMemcpyHostToDevice, copy_stream_));
+      cudaEvent_t ev = chunk_event(k);
       CK(cudaEventRecord(ev, copy_stream_));
       CK(cudaStreamWaitEvent(front_stream_, ev, 0));
-      const uint32_t cnt = last - first;
-      gk_tape_kernel<<<(cnt + kIngestThreads - 1) / kIngestThreads, kIngestThreads, 0, front_stream_>>>(f.in, first, cnt);
+      const uint32_t m = last - k;
+      gk_tape_kernel<<<(m + kIngestThreads - 1) / kIngestThreads, kIngestThreads, 0, front_stream_>>>(in, first + k, m);
       ++launches_;
-      first = last;
+      k = last;
     }
-    if (getenv("GK_TRACE_LAUNCH")) fprintf(stderr, "[launch] gk_tape_kernel over %u objects, after a host->device copy of %llu bytes\n", n, B);
-    if (n == 0) CK(cudaStreamWaitEvent(front_stream_, chunk_event_after_copy(), 0));
-    CK(cudaEventRecord(f.done, front_stream_));
-    f.pending = true;
-    return f;
+    if (getenv("GK_TRACE_LAUNCH"))
+      fprintf(stderr, "[launch] gk_tape_kernel over %u objects, after a host->device copy of %llu bytes\n", cnt, cnt ? ooff[cnt] - ooff[0] : 0ull);
+    if (cnt == 0) CK(cudaStreamWaitEvent(front_stream_, chunk_event_after_copy(), 0));
   }
   cudaEvent_t chunk_event_after_copy() {
     cudaEvent_t ev = chunk_event(0);

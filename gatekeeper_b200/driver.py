@@ -71,7 +71,7 @@ EXPORTS = [
     "gk_constraint_key", "gk_result_constraint_key", "gk_review_batch", "gk_batch_upload", "gk_batch_eval", "gk_batch_eval_device",
     "gk_batch_eval_device_peers", "gk_batch_upload_blob", "gk_review_blob", "gk_set_excluded_namespaces", "gk_audit_begin", "gk_audit_add_batch", "gk_audit_report",
     "gk_audit_end", "gk_validation_messages", "gk_host_cpus", "gk_pin_host", "gk_blob_prefetch", "gk_coalescer_create", "gk_coalescer_review", "gk_coalescer_stats",
-    "gk_coalescer_destroy", "gk_batch_size", "gk_batch_alg_bytes", "gk_batch_free", "gk_batch_refresh", "gk_free_result", "gk_free_str", "gk_dump",
+    "gk_coalescer_destroy", "gk_batch_size", "gk_batch_alg_bytes", "gk_batch_free", "gk_batch_refresh", "gk_batch_patch", "gk_free_result", "gk_free_str", "gk_dump",
     "gk_stat_description", "gk_audit_add_batch_ordered", "gk_audit_select_ms", "gk_audit_export", "gk_audit_merge",
 ]
 
@@ -149,6 +149,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.gk_batch_alg_bytes.argtypes = [P]
     lib.gk_batch_free.argtypes = [P, P]
     lib.gk_batch_refresh.argtypes = [P, P, C.POINTER(gk_result), PP]
+    lib.gk_batch_patch.argtypes = [P, P, C.POINTER(C.c_uint32), C.c_size_t, P, C.POINTER(C.c_uint64), C.c_size_t, C.POINTER(gk_result), PP]
     lib.gk_free_result.argtypes = [C.POINTER(gk_result)]
     lib.gk_free_str.argtypes = [C.c_void_p]
     lib.gk_dump.restype = C.c_void_p
@@ -693,6 +694,26 @@ class ResidentBatch:
         if rc == 1:
             self.stats = out
         return dict(out, rebuilt=rc == 1)
+
+    def patch(self, drop: Sequence[int], docs) -> dict:
+        """gk_batch_patch: the objects at indices `drop` leave the batch and `docs` (a workloads.ObjectBlob, or a list of JSON
+        documents as bytes) are appended after the objects that stay; the batch is then what an upload of that page would be under the
+        current constraint set.  The batch must have been uploaded with keep_source=True.  It keeps a reference to every page it
+        was given, since the engine reads the objects' JSON from where it was handed over.  Returns the call's statistics and the
+        new size as "n"."""
+        import numpy as np
+        from . import workloads as W
+        page = docs if hasattr(docs, "offsets") else W.PyBlob(list(docs))
+        idx = np.ascontiguousarray(list(drop) if not isinstance(drop, np.ndarray) else drop, dtype=np.uint32)
+        stats = gk_result()
+        err = C.c_char_p()
+        rc = self.drv._lib.gk_batch_patch(self.drv._e, self.h, idx.ctypes.data_as(C.POINTER(C.c_uint32)), len(idx), page.buf if len(page) else None,
+                                          page.offsets if len(page) else None, len(page), C.byref(stats), C.byref(err))
+        if rc < 0:
+            self.drv._check(rc, err)
+        self._keep = (self._keep, page)
+        self.stats = {"flatten_ms": stats.flatten_ms, "h2d_ms": stats.h2d_ms, "h2d_bytes": stats.h2d_bytes, "alg_bytes": stats.alg_bytes}
+        return dict(self.stats, kernel_ms=stats.kernel_ms, n=rc)
 
     def free(self):
         if self.h:

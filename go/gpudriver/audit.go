@@ -139,6 +139,44 @@ func (d *Driver) RefreshBatch(b *C.gk_batch_t) error {
 	return nil
 }
 
+// PatchBatch replaces objects of a resident page uploaded with GK_F_KEEP_SOURCE (gk_batch_patch): the objects at indices `drop`
+// leave it and `docs` are appended after the objects that stay, which keep their order; the batch is then what an upload of that
+// page would be under the current constraint set.  The staying objects are neither sent nor tokenised again.  An updated object is
+// dropped and its new version added.  The documents are copied into one C page, returned: the engine reads the objects' JSON from it
+// for messages and the audit, so the caller frees it (C.free) only when none of its objects is in the batch any more, or after the
+// batch is freed.  On error the batch is unchanged and no page is returned.
+func (d *Driver) PatchBatch(b *C.gk_batch_t, drop []uint32, docs [][]byte) (unsafe.Pointer, int, error) {
+	d.mux.RLock()
+	defer d.mux.RUnlock()
+	total := 0
+	for _, doc := range docs {
+		total += len(doc)
+	}
+	page := C.malloc(C.size_t(total + 1))
+	offs := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(len(docs)+1) * 8))[: len(docs)+1 : len(docs)+1]
+	defer C.free(unsafe.Pointer(&offs[0]))
+	dst := (*[1 << 40]byte)(page)[:total:total]
+	pos := 0
+	for i, doc := range docs {
+		offs[i] = C.uint64_t(pos)
+		pos += copy(dst[pos:], doc)
+	}
+	offs[len(docs)] = C.uint64_t(pos)
+	var cdrop *C.uint32_t
+	if len(drop) > 0 {
+		cdrop = (*C.uint32_t)(C.malloc(C.size_t(len(drop)) * 4))
+		defer C.free(unsafe.Pointer(cdrop))
+		copy((*[1 << 30]uint32)(unsafe.Pointer(cdrop))[:len(drop):len(drop)], drop)
+	}
+	var cerr *C.char
+	rc := C.gk_batch_patch(d.e, b, cdrop, C.size_t(len(drop)), (*C.char)(page), &offs[0], C.size_t(len(docs)), nil, &cerr)
+	if rc < 0 {
+		C.free(page)
+		return nil, 0, takeErr(cerr)
+	}
+	return page, int(rc), nil
+}
+
 func (r *AuditRun) Report() (*AuditReport, error) {
 	var cerr *C.char
 	js := C.gk_audit_report(r.a, &cerr)

@@ -208,6 +208,23 @@ void gk_batch_free(gk_engine_t* e, gk_batch_t* b);
  * negative on error -- then the batch is unchanged, still on its old constraint set.  `stats` (may be NULL): flatten_ms, h2d_ms,
  * h2d_bytes, alg_bytes as for an upload. */
 int gk_batch_refresh(gk_engine_t* e, gk_batch_t* b, gk_result* stats, char** err);
+/* Replace the object set of a resident batch uploaded with gk_batch_upload_blob(..., GK_F_KEEP_SOURCE): the objects at indices
+ * `drop` (indices of the batch before the call, any order) leave it, and the n_add documents of `buf` / `offsets` (as for
+ * gk_batch_upload_blob) are appended after the objects that stay, which keep their relative order.  Afterwards the batch is what
+ * gk_batch_upload_blob of (the staying objects in order, then the new ones) with the upload's source and flags would be, under the
+ * engine's current constraint set, excluder and ExpansionTemplates -- so it also does what gk_batch_refresh does.  The staying
+ * objects are neither copied from the host nor tokenised again: their JSON and token tape move within the kept device page, only the
+ * added documents are copied and tokenised, and then every column is extracted again over the new page.  To replace an object, drop
+ * it and add its new version.  Returns the new gk_batch_size, or negative on error: an index out of range or given twice, a batch
+ * without a kept source -> GK_ERR_INVALID; then the batch is unchanged.  `stats` as for gk_batch_refresh (may be NULL); kernel_ms is
+ * the device time of the splice, the added documents' copy and tokeniser, and the extraction.
+ * A batch keeps no device source when its constraint set was flattened on the host at upload (referential sets, Dump's "ingest: host
+ * flattener (...)"); the call refuses it (GK_ERR_INVALID, with a text that says so), and it refuses every batch while the current
+ * constraint set is flattened on the host: a patch never flattens on the host -- upload the page again instead.
+ * The host still reads the objects' JSON for messages, the audit and expansion, where it was given: `buf` must stay alive while the
+ * batch lives, as must the pages of the upload and of earlier patches that hold objects still in the batch. */
+int gk_batch_patch(gk_engine_t* e, gk_batch_t* b, const uint32_t* drop, size_t n_drop, const char* buf, const uint64_t* offsets,
+                   size_t n_add, gk_result* stats, char** err);
 
 /* ---- stage-0 excluder: Config.spec.match[].excludedNamespaces of one process ("audit", "webhook", "sync",
  * "mutation-webhook", or "*" = all four), pkg/controller/config/process/excluder.go:53-127.  Replaces the process' set.
