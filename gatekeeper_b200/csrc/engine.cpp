@@ -2116,7 +2116,11 @@ void Engine::lut_fill(const Compiled& c, const uint8_t* blob, const GkMiss* miss
           switch (ma.kind) {
             case GK_ARG_JSON: vals[a] = json_parse(reinterpret_cast<const char*>(blob) + ma.off, ma.len); break;
             case GK_ARG_INDEX: vals[a] = v_int((long long)ma.off); break;
-            case GK_ARG_SYNSTR: vals[a] = v_str(std::string(ma.len ? reinterpret_cast<const char*>(blob) + ma.off : "", ma.len)); break;
+            case GK_ARG_SYNSTR: {   // a JSON string body: a slice of an escaped apiVersion keeps its escapes
+              std::string s(ma.len ? reinterpret_cast<const char*>(blob) + ma.off : "", ma.len);
+              vals[a] = s.find('\\') == std::string::npos ? v_str(std::move(s)) : json_parse(("\"" + s + "\"").data(), s.size() + 2);
+              break;
+            }
             default: break;
           }
         }

@@ -352,8 +352,9 @@ GK_HD gk_u64 gk_hash_bytes(gk_u64 h, const uint8_t* p, uint32_t n) {
 struct GkXVal {
   uint32_t vt;          // GK_VT_*
   uint32_t node;        // tape index, GK_NONE for synthetic values
-  const uint8_t* sp;    // synthetic string: decoded bytes
+  const uint8_t* sp;    // synthetic string: the bytes of a JSON string body (decoded bytes unless `sesc`)
   uint32_t slen;
+  uint32_t sesc;        // the synthetic string may hold escapes (a slice of an escaped apiVersion): read it through gk_x_str
   long long inum;       // synthetic number (array index)
 };
 GK_HD GkXVal gk_xundef() {
@@ -362,6 +363,7 @@ GK_HD GkXVal gk_xundef() {
   v.node = GK_NONE;
   v.sp = nullptr;
   v.slen = 0;
+  v.sesc = 0;
   v.inum = 0;
   return v;
 }
@@ -375,6 +377,11 @@ GK_HD GkXVal gk_xstr(const uint8_t* p, uint32_t n) {
   v.vt = GK_VT_STR;
   v.sp = p;
   v.slen = n;
+  return v;
+}
+GK_HD GkXVal gk_xstr_esc(const uint8_t* p, uint32_t n, uint32_t esc) {
+  GkXVal v = gk_xstr(p, n);
+  v.sesc = esc;
   return v;
 }
 GK_HD uint32_t gk_vt_of_type(uint32_t t) {
@@ -439,6 +446,14 @@ GK_HD bool gk_entries_eq(const GkDoc& d, gk_u64 a, gk_u64 b) {
     if (cx != cy) return false;
     if (cx < 0) return true;
   }
+}
+
+// hash of a (decoded) string entry's bytes, continuing from h
+GK_HD gk_u64 gk_hash_entry(const GkDoc& d, gk_u64 e, gk_u64 h) {
+  if (!gk_te_esc(e)) return gk_hash_bytes(h, d.js + gk_te_off(e), gk_te_len(e));
+  GkStr s = gk_str_open(d.js + gk_te_off(e), gk_te_len(e));
+  for (int b; (b = gk_str_next(s)) >= 0;) h = gk_hash_byte(h, (uint32_t)b);
+  return h;
 }
 
 // member lookup: the value index of key `lit` in the object at `node`, or GK_NONE.  A repeated key means its LAST value
@@ -588,7 +603,7 @@ enum { GK_ARG_UNDEF = 0, GK_ARG_JSON = 1, GK_ARG_INDEX = 2, GK_ARG_SYNSTR = 3 };
 typedef struct {
   uint32_t kind;
   uint32_t len;
-  unsigned long long off;   // GK_ARG_JSON: absolute offset in the blob; GK_ARG_INDEX: the index; GK_ARG_SYNSTR: absolute offset of the decoded bytes
+  unsigned long long off;   // GK_ARG_JSON: absolute offset in the blob; GK_ARG_INDEX: the index; GK_ARG_SYNSTR: absolute offset of a JSON string body's bytes (the host decodes any escapes)
 } GkMissArg;
 #define GK_LUT_MAX_ARGS 4
 typedef struct {
@@ -726,10 +741,11 @@ struct GkXCtx {
   // review envelope
   uint32_t env_ready;            // gk_x_envelope has run
   uint32_t api_node, kind_node, name_node, ns_node, meta_node;   // tape indices or GK_NONE
-  const uint8_t* grp;            // group / version slices of apiVersion (raw, apiVersion has no escapes in the supported case)
-  uint32_t grp_len;
+  const uint8_t* grp;            // group / version slices of the raw apiVersion, cut at its first decoded '/'; each holds whole
+  uint32_t grp_len;              // escapes only
   const uint8_t* ver;
   uint32_t ver_len;
+  uint32_t env_esc;              // apiVersion holds escapes: the slices are read decoded (gk_x_str)
   // current row of every scope on the DFS stack
   // (kept small: this context lives in per-thread local memory, and ncu showed the column pass bound by local-memory misses --
   // 4 GB of them per 1.6 M rows -- when each depth held two 32-byte values)
@@ -752,13 +768,35 @@ GK_HD void gk_x_envelope(GkXCtx& c) {
   c.kind_node = gk_obj_find(c.doc, 0, reinterpret_cast<const uint8_t*>("kind"), 4);
   c.grp = c.ver = nullptr;
   c.grp_len = c.ver_len = 0;
+  c.env_esc = 0;
   if (c.api_node != GK_NONE && gk_te_type(c.doc.tape[c.api_node]) == GK_T_STR) {
     const gk_u64 e = c.doc.tape[c.api_node];
     const uint8_t* p = c.doc.js + gk_te_off(e);
     const uint32_t len = gk_te_len(e);
-    uint32_t s = 0;
-    while (s < len && p[s] != '/') ++s;
-    if (s == len) {
+    uint32_t s = 0, w = 1;   // the separator: its raw offset and width ('/', or the escapes "\/" and 'u' 002F)
+    if (!gk_te_esc(e)) {
+      while (s < len && p[s] != '/') ++s;
+    } else {
+      // the tokeniser has checked every escape: a backslash is followed by one character, or by 'u' and four hex digits, inside
+      // the string.  Escapes are stepped over whole, so neither slice ends inside one.
+      c.env_esc = 1;
+      while (s < len && p[s] != '/') {
+        if (p[s] != '\\') {
+          ++s;
+        } else if (p[s + 1] == '/') {
+          w = 2;
+          break;
+        } else if (p[s + 1] != 'u') {
+          s += 2;
+        } else if (gk_str_hex4(p + s + 2) == 0x2Fu) {
+          w = 6;
+          break;
+        } else {
+          s += 6;
+        }
+      }
+    }
+    if (s >= len) {
       c.ver = p;
       c.ver_len = len;
       c.grp = p;
@@ -766,8 +804,8 @@ GK_HD void gk_x_envelope(GkXCtx& c) {
     } else {
       c.grp = p;
       c.grp_len = s;
-      c.ver = p + s + 1;
-      c.ver_len = len - s - 1;
+      c.ver = p + s + w;
+      c.ver_len = len - s - w;
     }
   }
   c.meta_node = gk_obj_find(c.doc, 0, reinterpret_cast<const uint8_t*>("metadata"), 8);
@@ -825,8 +863,8 @@ GK_HD GkXVal gk_x_root(const GkXCtx& cc, uint32_t root, const uint32_t* keys, ui
       const uint8_t* k = c.xp->xbytes + keys[1];
       const uint32_t kl = keys[2];
       if (gk_lit_eq(k, kl, "kind")) return c.kind_node != GK_NONE ? gk_xnode(c.doc.tape, c.kind_node) : gk_xstr(nullptr, 0);
-      if (gk_lit_eq(k, kl, "group")) return gk_xstr(c.grp, c.grp_len);
-      if (gk_lit_eq(k, kl, "version")) return gk_xstr(c.ver, c.ver_len);
+      if (gk_lit_eq(k, kl, "group")) return gk_xstr_esc(c.grp, c.grp_len, c.env_esc);
+      if (gk_lit_eq(k, kl, "version")) return gk_xstr_esc(c.ver, c.ver_len, c.env_esc);
       return gk_xundef();
     }
     case GK_R_NAME:
@@ -983,7 +1021,7 @@ GK_HD GkStr gk_x_str(const GkXCtx& c, const GkXVal& v) {
     const gk_u64 e = c.doc.tape[v.node];
     return gk_str_open(c.doc.js + gk_te_off(e), gk_te_len(e));
   }
-  return gk_str_open(v.sp, v.slen);   // synthetic strings hold decoded bytes without backslashes
+  return gk_str_open(v.sp, v.slen);   // synthetic strings are JSON string bodies: decoded bytes without backslashes, or `sesc`
 }
 
 GK_HD uint32_t gk_x_sid_exotic(const GkXCtx& c, const GkXVal& v);
@@ -1174,6 +1212,7 @@ GK_HD bool gk_sx_run(const GkXCtx& c, const GkXClosure& cl, GkSV* out) {
           x.p = c.doc.js + gk_te_off(e);
           x.len = gk_te_len(e);
         } else {
+          if (v.sesc) return false;
           x.p = v.sp;
           x.len = v.slen;
         }
@@ -1253,10 +1292,13 @@ GK_HD bool gk_sx_run(const GkXCtx& c, const GkXClosure& cl, GkSV* out) {
 
 // ---------------------------------------------------------------------------------------------- one object
 GK_HD uint32_t gk_decoded_len(const GkXCtx& c, const GkXVal& v) {
-  if (v.node == GK_NONE) return v.slen;
-  const gk_u64 e = c.doc.tape[v.node];
-  if (!gk_te_esc(e)) return gk_te_len(e);
-  GkStr s = gk_str_open(c.doc.js + gk_te_off(e), gk_te_len(e));
+  if (v.node == GK_NONE) {
+    if (!v.sesc) return v.slen;
+  } else {
+    const gk_u64 e = c.doc.tape[v.node];
+    if (!gk_te_esc(e)) return gk_te_len(e);
+  }
+  GkStr s = gk_x_str(c, v);
   uint32_t n = 0;
   while (gk_str_next(s) >= 0) ++n;
   return n;
@@ -1425,7 +1467,7 @@ GK_HD void gk_ingest_obj(const GkXProg& xp, const GkIngestIn& in, const GkIngest
       if (ns != GK_NONE) fl |= GK_F_HAS_NS;
       if (MODE == GK_PASS_HEADER) {
         kind_sid = gk_x_sid(c, kindv);
-        group_sid = gk_x_sid(c, gk_xstr(c.grp, c.grp_len));
+        group_sid = gk_x_sid(c, gk_xstr_esc(c.grp, c.grp_len, c.env_esc));
       }
       if (ns != GK_NONE) {   // the Namespace object of the review: the cache entry for the object's namespace (matcher.go:37-39)
         GkStr s = gk_x_str(c, gk_xnode(c.doc.tape, ns));
@@ -1454,14 +1496,11 @@ GK_HD void gk_ingest_obj(const GkXProg& xp, const GkIngestIn& in, const GkIngest
       if (out.gvk) {
         gk_u64 hh = 0;
         if (!skip) {
+          // of the decoded strings, so that spellings of one (apiVersion, kind) share the hash
           hh = 0x9ae16a3b2f90404full;
-          if (c.api_node != GK_NONE && gk_te_type(c.doc.tape[c.api_node]) == GK_T_STR) {
-            const gk_u64 e = c.doc.tape[c.api_node];
-            hh = gk_hash_bytes(hh, c.doc.js + gk_te_off(e), gk_te_len(e));
-          }
+          if (c.api_node != GK_NONE && gk_te_type(c.doc.tape[c.api_node]) == GK_T_STR) hh = gk_hash_entry(c.doc, c.doc.tape[c.api_node], hh);
           hh = gk_hash_byte(hh, 0xFFu);
-          const gk_u64 ek = c.doc.tape[c.kind_node];
-          hh = gk_hash_fin(gk_hash_bytes(hh, c.doc.js + gk_te_off(ek), gk_te_len(ek))) | 1ull;
+          hh = gk_hash_fin(gk_hash_entry(c.doc, c.doc.tape[c.kind_node], hh)) | 1ull;
         }
         out.gvk[i] = hh;
       }
