@@ -109,9 +109,19 @@ struct IdView {
 };
 }  // namespace
 
+bool HostCandidates::operator()(uint32_t o, uint32_t c) const { return thr_all[c] || IdView{*id}.cmp(o, thr_obj[c]) <= 0; }
+
+void AuditRun::add_counted(const std::string& key, const std::string& action, uint64_t n) {
+  auto& pc = per_constraint[key];
+  pc.queue.limit = limit;
+  pc.total += n;
+  by_action[action] += n;
+  results += n;
+}
+
 void AuditRun::add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn>& objs, const uint32_t* viol, const uint32_t* err,
                          uint32_t words, const std::vector<uint32_t>& errlist, const std::string& ep, const BatchIdentity* id, const uint32_t* amb,
-                         const uint32_t* cand) {
+                         const uint32_t* cand, HostCandidates* keep) {
   const size_t n = objs.size();
   const uint32_t C = (uint32_t)c.order.size();
   // ---- lazy path: which pairs need the host at all
@@ -167,6 +177,12 @@ void AuditRun::add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn
       thr_obj[cix] = all[limit - 1];
       thr_all[cix] = 0;
     }
+  }
+  if (keep) {
+    keep->lazy = lazy && limit && !cand;
+    keep->id = id;
+    keep->thr_obj = thr_obj;
+    keep->thr_all = thr_all;
   }
   std::unordered_map<uint64_t, uint32_t> err_code;
   for (size_t i = 0; i + 2 < errlist.size(); i += 3) err_code[((uint64_t)errlist[i] << 32) | errlist[i + 1]] = errlist[i + 2];
@@ -245,11 +261,7 @@ void AuditRun::add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn
     for (uint32_t cix = 0; cix < C; ++cix)
       if (counted[cix]) {
         const Constraint& con = *c.order[cix];
-        auto& pc = part.per_constraint[con.kind + "/" + con.name];
-        pc.queue.limit = limit;
-        pc.total += counted[cix];
-        part.by_action[con.action] += counted[cix];
-        part.results += counted[cix];
+        part.add_counted(con.kind + "/" + con.name, con.action, counted[cix]);
         part.counted_pairs += counted[cix];
       }
   };
@@ -266,9 +278,9 @@ void AuditRun::add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn
 }
 
 // Backend::audit_candidates on the host: the flagged objects sorted by (group, version, kind, namespace, name), then per constraint
-// the rank of its limit-th flagged object bounds its candidates.
+// the rank of its limit-th flagged object bounds its candidates.  With `keep`, every object is ranked, flagged or not.
 void Backend::audit_candidates(void* batch, const uint32_t* viol, uint32_t words, uint32_t nconstraints, uint32_t limit, const GvkOf& gvk_of,
-                               std::vector<uint32_t>& cand, float* device_ms) {
+                               std::vector<uint32_t>& cand, float* device_ms, AuditRanks* keep) {
   if (device_ms) *device_ms = 0.f;
   BatchIdentity id;
   identity(batch, id);
@@ -281,13 +293,16 @@ void Backend::audit_candidates(void* batch, const uint32_t* viol, uint32_t words
     std::string g, v, k;
   };
   std::vector<Flagged> fl;
-  for (uint32_t o = 0; o < n; ++o)
+  auto flagged = [&](uint32_t o) {
     for (uint32_t cix = 0; cix < nconstraints; ++cix)
-      if (bit(o, cix)) {
-        fl.push_back({o, {}, {}, {}});
-        gvk_of(o, fl.back().g, fl.back().v, fl.back().k);
-        break;
-      }
+      if (bit(o, cix)) return true;
+    return false;
+  };
+  for (uint32_t o = 0; o < n; ++o)
+    if (keep || flagged(o)) {
+      fl.push_back({o, {}, {}, {}});
+      gvk_of(o, fl.back().g, fl.back().v, fl.back().k);
+    }
   auto cmp = [&](const Flagged& a, const Flagged& b) {
     if (a.g != b.g) return a.g < b.g ? -1 : 1;
     if (a.v != b.v) return a.v < b.v ? -1 : 1;
@@ -297,12 +312,19 @@ void Backend::audit_candidates(void* batch, const uint32_t* viol, uint32_t words
   std::sort(fl.begin(), fl.end(), [&](const Flagged& a, const Flagged& b) { return cmp(a, b) < 0; });
   std::vector<uint32_t> rank(fl.size(), 0);
   for (size_t p = 1; p < fl.size(); ++p) rank[p] = rank[p - 1] + (cmp(fl[p - 1], fl[p]) != 0);
+  if (keep) {
+    keep->rank.assign(n, 0);
+    keep->thr.assign(nconstraints, ~0u);
+    keep->dev.reset();
+    for (size_t p = 0; p < fl.size(); ++p) keep->rank[fl[p].o] = rank[p];
+  }
   for (uint32_t cix = 0; cix < nconstraints; ++cix) {
     uint32_t seen = 0, thr = ~0u;
     for (size_t p = 0; p < fl.size() && thr == ~0u; ++p)
       if (bit(fl[p].o, cix) && ++seen == limit) thr = rank[p];
     for (size_t p = 0; p < fl.size() && rank[p] <= thr; ++p)
       if (bit(fl[p].o, cix)) cand[(size_t)fl[p].o * words + (cix >> 5)] |= 1u << (cix & 31u);
+    if (keep) keep->thr[cix] = thr;
   }
 }
 

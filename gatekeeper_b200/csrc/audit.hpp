@@ -26,6 +26,16 @@ struct LimitQueue {
   std::vector<StatusViolation> drain_descending();
 };
 
+// The host threshold scan's candidate rule, as one add_batch over a page of one kind computed it: object o (identity in `id`) can still
+// enter constraint c's list.  `lazy`: the scan ran; otherwise add_batch rendered every pair and there is no rule.
+struct HostCandidates {
+  bool lazy = false;
+  const BatchIdentity* id = nullptr;
+  std::vector<uint32_t> thr_obj;
+  std::vector<uint8_t> thr_all;
+  bool operator()(uint32_t o, uint32_t c) const;
+};
+
 struct AuditRun {
   size_t limit = 20;      // --constraint-violations-limit (manager.go:64)
   size_t msg_size = 256;  // msgSize (manager.go:48)
@@ -55,8 +65,14 @@ struct AuditRun {
   void add_batch(Engine& eng, const Compiled& c, const std::vector<ObjIn>& objs, const uint32_t* viol, const uint32_t* err,
                  uint32_t words, const std::vector<uint32_t>& errlist, const std::string& ep, const BatchIdentity* id = nullptr,
                  const uint32_t* amb = nullptr,    // amb: the ambiguity netlist's bitmap (bit clear = at most one result for the pair)
-                 const uint32_t* cand = nullptr);  // cand: the candidate bitmap [n * words]
+                 const uint32_t* cand = nullptr,   // cand: the candidate bitmap [n * words]
+                 HostCandidates* keep = nullptr);  // keep: receives the threshold scan's rule (with `id`)
   uint64_t rendered_pairs = 0, counted_pairs = 0;   // pairs evaluated on the host / taken from the bitmap (lazy path)
+  // `n` results of constraint `key` (enforcement action `action`) counted from the bitmap: in the totals, no status list entry
+  void add_counted(const std::string& key, const std::string& action, uint64_t n);
+  // An expanded batch's resultant violation pairs rendered on the host / counted from the bitmap (gk_audit_resultant_pairs).  Kept
+  // apart from the two above, which count the parents' pairs only; not exported: they cover the batches added to this run.
+  uint64_t resultant_rendered = 0, resultant_counted = 0;
   std::string report();
   // The run's partial state as a versioned byte string (gk_audit_export), and its inverse: parse() fills an empty run or throws
   // RegoError on a truncated, corrupted or foreign buffer.

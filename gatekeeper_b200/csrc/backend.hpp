@@ -84,6 +84,26 @@ struct BatchIdentity {
   std::vector<uint8_t> ns_bytes, name_bytes;
 };
 
+// The ranking of one audit_candidates call, kept for audit_resultants: rank[o], the rank of object o's identity (equal identities share
+// one), and thr[c], the rank of constraint c's limit-th flagged object (~0u: fewer than `limit` are flagged).  The CUDA backend keeps
+// both on the device, in `dev`; the host default keeps them in the vectors.
+struct AuditRanks {
+  std::vector<uint32_t> rank, thr;
+  std::shared_ptr<void> dev;
+};
+
+// An expanded batch's resultants as the audit sorts their pairs (fold_core.h gk_classify_resultant).
+struct ResultantSplit {
+  std::vector<uint64_t> counted;   // [classes * nconstraints] pairs counted, per action class (ResultantClasses::cls) and constraint
+  std::vector<uint32_t> render;    // the pairs to render, (resultant, constraint | is_err << 31) each, in no particular order
+};
+struct ResultantClasses {
+  const uint8_t* single = nullptr;   // [nconstraints] Compiled::single_result
+  const uint8_t* cls = nullptr;      // [resultants] action class: 0 = the constraint's own action, k = the k-th template override
+  uint32_t classes = 1, nconstraints = 0, parents = 0;
+  const uint8_t* dead = nullptr;     // [parents] 1: the parent's own review failed, its resultants take no part (null: none)
+};
+
 class Backend {
  public:
   virtual ~Backend() {}
@@ -123,10 +143,19 @@ class Backend {
   // candidates are the objects whose bit c is set in `viol` [n * words] and whose identity is at or below the `limit`-th smallest
   // such identity, ties included (all of them when fewer than `limit` are set).  `cand` receives that bitmap [n * words].  `gvk_of`
   // decodes the (group, version, kind) of one object from its JSON: the backend asks for one object of each distinct apiVersion /
-  // kind it holds.  The CUDA backend ranks and selects on the device; this default does it on the host from identity().
+  // kind it holds.  The CUDA backend ranks and selects on the device; this default does it on the host from identity().  `keep` (may be
+  // null) receives the ranking for audit_resultants.
   using GvkOf = std::function<void(uint32_t object, std::string& group, std::string& version, std::string& kind)>;
   virtual void audit_candidates(void* batch, const uint32_t* viol, uint32_t words, uint32_t nconstraints, uint32_t limit, const GvkOf& gvk_of,
-                                std::vector<uint32_t>& cand, float* device_ms);
+                                std::vector<uint32_t>& cand, float* device_ms, AuditRanks* keep = nullptr);
+  // The audit of an expanded batch's resultants against their parents' ranking `ranks` (audit_candidates of the parent batch): pair
+  // (r, c) is counted when it is a violation with one result (`cls.single`, or a clear bit of the ambiguity plane) and r's parent p
+  // is above c's threshold (rank[p] > thr[c]); every other flagged pair is listed in `out.render`.  `res` is the resultant batch as
+  // its last eval() left it, `amb` its ambiguity fork as its last eval() left it (may be null), with the CSR (par, off) of set_parents.
+  // The CUDA backend reads the planes the evaluations left on the device; this default reads the host planes of `rev` / `ramb`.
+  virtual void audit_resultants(void* res, void* amb, const EvalOut& rev, const EvalOut* ramb, const std::vector<uint32_t>& par,
+                                const std::vector<uint32_t>& off, const AuditRanks& ranks, const ResultantClasses& cls, ResultantSplit& out,
+                                float* device_ms);
   // ---- expanded batches (GK_F_EXPAND, gk_engine.h).  The defaults run on the host: for a backend whose batches are host memory and
   // whose "device" output buffers are host memory too (the test-only host emulation).
   // Generator selection: the objects of `batch` that may have resultants, ascending, into `sel`: those whose (group, version, kind)
@@ -246,6 +275,40 @@ inline void fold_host(const GkFoldArgs& a) {
       a.peer_tot[q][c] = a.totals[c];
       a.peer_tot[q][a.tot_stride + c] = a.err_totals[c];
     }
+}
+
+// gk_classify_resultant over every resultant of the CSR (par, off) on host planes; `cand(p, c)`: parent p can still enter constraint c's list
+template <class Cand>
+inline void classify_resultants_host(const GkResClassArgs& a, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off,
+                                     const ResultantClasses& cls, Cand&& cand, ResultantSplit& out) {
+  if (off.size() != par.size() + 1) throw BackendError{"audit resultants: the offsets must have one entry more than the parents"};
+  const uint32_t C = cls.nconstraints;
+  out.counted.assign((size_t)cls.classes * C, 0);
+  out.render.clear();
+  for (size_t j = 0; j < par.size(); ++j) {
+    const uint32_t p = par[j];
+    if (cls.dead && cls.dead[p]) continue;
+    for (uint32_t r = off[j]; r < off[j + 1]; ++r)
+      gk_classify_resultant(
+          a, r, [&](uint32_t c) { return cand(p, c); }, [&](uint32_t c) { ++out.counted[(size_t)cls.cls[r] * C + c]; },
+          [&](uint32_t c, uint32_t is_err) { out.render.insert(out.render.end(), {r, c | is_err << 31}); });
+  }
+}
+
+inline void Backend::audit_resultants(void* res, void* amb, const EvalOut& rev, const EvalOut* ramb, const std::vector<uint32_t>& par,
+                                      const std::vector<uint32_t>& off, const AuditRanks& ranks, const ResultantClasses& cls, ResultantSplit& out,
+                                      float* device_ms) {
+  (void)res, (void)amb;
+  if (device_ms) *device_ms = 0.f;
+  if (!off.empty() && (size_t)off.back() * rev.words > rev.viol.size()) throw BackendError{"audit resultants: more resultants than the planes hold"};
+  GkResClassArgs a{};
+  a.viol = rev.viol.data();
+  a.err = rev.err.data();
+  a.amb = ramb ? ramb->viol.data() : nullptr;
+  a.single = cls.single;
+  a.words = rev.words;
+  a.nconstraints = cls.nconstraints;
+  classify_resultants_host(a, par, off, cls, [&](uint32_t p, uint32_t c) { return ranks.rank[p] <= ranks.thr[c]; }, out);
 }
 
 inline void Backend::select_generators(void* batch, const GvkOf& gvk_of, const GvkWanted& wanted, std::vector<uint32_t>& sel, uint32_t* kinds,

@@ -1165,7 +1165,7 @@ int gk_set_excluded_namespaces(gk_engine_t* e, const char* process, const char* 
 struct gk_audit {
   gk_engine* e;
   AuditRun run;
-  float select_ms = 0.f;   // device time of the last gk_audit_add_batch_ordered's ranking and selection
+  float select_ms = 0.f;   // device time of the last gk_audit_add_batch_ordered's ranking, selection and resultant classification
 };
 
 gk_audit_t* gk_audit_begin(gk_engine_t* e, uint32_t violations_limit, uint32_t msg_size, char** err) {
@@ -1179,6 +1179,48 @@ gk_audit_t* gk_audit_begin(gk_engine_t* e, uint32_t violations_limit, uint32_t m
   return a;
 }
 
+namespace {
+// The results `vio` of resultants (object k: children[k]) entered into `run` as results of their parents (parent i's JSON: ins[i]) --
+// addAuditResponsesToUpdateLists names the parent object: "[Implied by <template>]", the template's enforcement-action override
+void fold_resultant_results(AuditRun& run, const Compiled& c, const std::vector<Violation>& vio, const std::vector<Child>& children,
+                            const std::vector<ObjIn>& ins) {
+  struct Ident {
+    std::string g, v, k, ns, name;
+  };
+  std::unordered_map<uint32_t, Ident> ident;   // parents that have results from resultants, parsed once each
+  for (auto& v : vio) {
+    const Child& ch = children[v.object];
+    auto it = ident.find(ch.parent);
+    if (it == ident.end()) {
+      Ident id2;
+      try {
+        VP po = json_parse(ins[ch.parent].json, ins[ch.parent].len);
+        split_gv(po, id2.g, id2.v, id2.k);
+        id2.ns = meta_str(po, "namespace");
+        id2.name = meta_str(po, "name");
+      } catch (JsonError&) {
+      }
+      it = ident.emplace(ch.parent, std::move(id2)).first;
+    }
+    const Constraint& con = *c.order[v.constraint];
+    StatusViolation sv;
+    sv.group = it->second.g, sv.version = it->second.v, sv.kind = it->second.k, sv.ns = it->second.ns, sv.name = it->second.name;
+    sv.message = ExpansionSystem::implied_by(ch.tmpl, v.msg);
+    sv.action = ch.action.empty() ? v.action : ch.action;   // OverrideEnforcementAction: the action only
+    sv.scoped_json = v.scoped_json;
+    run.fold(con.kind + "/" + con.name, std::move(sv));
+    run.results++;
+  }
+}
+
+// a resultant the review refused (manager.go:757-760 logs it and goes on): reported on its parent, unless the parent has an error
+void resultant_errors(std::vector<std::string>& obj_errs, const std::vector<std::string>& res_errors, const std::vector<Child>& children) {
+  for (size_t k = 0; k < res_errors.size() && k < children.size(); ++k)
+    if (!res_errors[k].empty() && obj_errs[children[k].parent].empty())
+      obj_errs[children[k].parent] = ExpansionSystem::implied_by(children[k].tmpl, res_errors[k]);
+}
+}  // namespace
+
 // gk_audit_add_batch and gk_audit_add_batch_ordered: `ordered` takes the lazy path's candidates from Backend::audit_candidates (any mix
 // of kinds) instead of the host threshold scan over (namespace, name), which only a page of one kind allows
 static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordered, char** err) {
@@ -1190,23 +1232,48 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
     std::string ep = ep_c ? ep_c : "";
     std::vector<uint32_t> active;
     e->eng->active_mask(*c, ep, active);
-    EvalOut ev, ev_amb;
+    // An expanded batch whose templates are current brings its resultants: they are not expanded again but evaluated where they are
+    // resident, their pairs sorted against the parents' candidates.  Its resultants must also be current for the constraint set,
+    // data.inventory and the excluder (the audit flattens re-expanded resultants with the current excluder).
+    const gk_batch* res = b->ex ? b->ex->res.get() : nullptr;
+    // action classes of the resultants: 0 = the constraint's own action, k > 0 = the k-th distinct template override
+    std::vector<std::string> actions(1);
+    std::vector<uint8_t> cls(res ? res->n : 0, 0);
+    for (size_t k = 0; k < cls.size() && actions.size() <= 256; ++k) {
+      const std::string& act = b->ex->x.children[k].action;
+      if (act.empty()) continue;
+      const size_t j = (size_t)(std::find(actions.begin(), actions.end(), act) - actions.begin());
+      if (j == actions.size()) actions.push_back(act);
+      cls[k] = (uint8_t)j;
+    }
+    const bool resident = b->ex && !expansion_stale(e, *b) && !getenv("GK_AUDIT_EAGER") && actions.size() <= 256 &&
+                          (!res || (!stale_reason(e, *c, *res) && excluded_of(e, res->flags) == res->excluded));
+    if (!resident) res = nullptr;
+    // The lazy path (audit.hpp): the namespace / name arrays of the batch and the bitmap of the ambiguity netlist let the run count
+    // the pairs that have exactly one result and evaluate only what can still enter a constraint's list.
+    const bool lazy = !getenv("GK_AUDIT_EAGER") && (c->amb || std::any_of(c->single_result.begin(), c->single_result.end(), [](uint8_t x) { return x != 0; }));
+    // (the ordered lazy path sorts the resultants' pairs on the device, from the planes their evaluation leaves there)
+    const bool res_on_device = ordered && lazy;
+    EvalOut ev, ev_amb, rev, rev_amb;
     {
       ProgramLease lease(e, *c);
       e->be->eval(b->dev.get(), active, ev, true);
+      if (res) e->be->eval(res->dev.get(), active, rev, !res_on_device);   // (unfolded: each resultant's pairs are counted on their own)
     }
     std::vector<ObjIn> ins(b->n);
     for (size_t i = 0; i < ins.size(); ++i) ins[i] = b->obj_in(i);
-    // The lazy path (audit.hpp): the namespace / name arrays of the batch and the bitmap of the ambiguity netlist let the run count
-    // the pairs that have exactly one result and evaluate only what can still enter a constraint's list.
     BatchIdentity id;
-    const bool lazy = !getenv("GK_AUDIT_EAGER") && (c->amb || std::any_of(c->single_result.begin(), c->single_result.end(), [](uint8_t x) { return x != 0; }));
     if (lazy && !ordered) e->be->identity(b->dev.get(), id);
     const bool use_amb = lazy && (ordered || id.uniform_gvk) && c->amb && !getenv("GK_AUDIT_NO_AMB");
+    BackendHandle res_fork;   // the resultants' ambiguity fork: its planes stay on the device for Backend::audit_resultants
     if (use_amb) {
       ProgramLease lease(e, *c->amb);   // (the backend holds one netlist at a time: waits until no review uses the other)
       BackendHandle fork = device_batch(e, e->be->fork_batch(b->dev.get(), *c->amb));
       e->be->eval(fork.get(), active, ev_amb, true);
+      if (res) {
+        res_fork = device_batch(e, e->be->fork_batch(res->dev.get(), *c->amb));
+        e->be->eval(res_fork.get(), active, rev_amb, !res_on_device);
+      }
     }
     // ---- expansion inside the audit loop (pkg/audit/manager.go:733-765): every reviewed object is expanded; its resultants are reviewed
     // as Generated resources with the parent's Namespace, their results -- "[Implied by <template>]", the template's action override --
@@ -1215,8 +1282,18 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
     std::vector<std::string> obj_errs = b->host->obj_errors.empty() ? std::vector<std::string>(b->n) : b->host->obj_errors;
     obj_errs.resize(b->n);
     // (an object whose own review failed is not expanded: the reference never gets to its expansion)
-    const Expansion x = e->eng->has_expansion() ? expand_page(*e->eng, ins, obj_errs, e->eng->threads()) : Expansion();
-    const std::vector<Child>& children = x.children;
+    Expansion x;
+    if (resident) {
+      for (size_t i = 0; i < b->ex->x.errors.size(); ++i)
+        if (obj_errs[i].empty()) x.errors.push_back(b->ex->x.errors[i]);
+        else x.errors.emplace_back();
+    } else if (e->eng->has_expansion()) {
+      const double t0 = now_ms();
+      x = expand_page(*e->eng, ins, obj_errs, e->eng->threads());
+      if (getenv("GK_TRACE_LAUNCH"))
+        fprintf(stderr, "[audit] expanded %u objects on the host: %zu resultants, %.3f ms\n", b->n, x.children.size(), now_ms() - t0);
+    }
+    const std::vector<Child>& children = resident ? b->ex->x.children : x.children;
     const uint32_t W = ev.words;
     for (size_t i = 0; i < x.errors.size(); ++i)
       if (!x.errors[i].empty()) {
@@ -1228,6 +1305,7 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
       }
     // (after the expansion above: the rows of objects whose expansion failed are cleared, and they are no candidates either)
     std::vector<uint32_t> cand;
+    AuditRanks ranks;   // the parents' ranking, kept for the resultants
     if (lazy && ordered) {
       auto gvk_of = [&ins](uint32_t o, std::string& g, std::string& v, std::string& k) {
         try {
@@ -1235,11 +1313,73 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
         } catch (JsonError&) {
         }
       };
-      e->be->audit_candidates(b->dev.get(), ev.viol.data(), ev.words, (uint32_t)c->order.size(), (uint32_t)a->run.limit, gvk_of, cand, &a->select_ms);
+      e->be->audit_candidates(b->dev.get(), ev.viol.data(), ev.words, (uint32_t)c->order.size(), (uint32_t)a->run.limit, gvk_of, cand, &a->select_ms,
+                              res ? &ranks : nullptr);
     }
+    HostCandidates hc;   // the host threshold scan's rule, kept for the resultants
     a->run.add_batch(*e->eng, *c, ins, ev.viol.data(), ev.err.empty() ? nullptr : ev.err.data(), ev.words, ev.errlist, ep,
-                     lazy && !ordered ? &id : nullptr, use_amb ? ev_amb.viol.data() : nullptr, lazy && ordered ? cand.data() : nullptr);
-    if (!children.empty()) {
+                     lazy && !ordered ? &id : nullptr, use_amb ? ev_amb.viol.data() : nullptr, lazy && ordered ? cand.data() : nullptr, &hc);
+    if (res) {
+      // ---- the resident resultants.  Their pairs are sorted against the parents' candidates (a resultant's results carry its
+      // parent's identity, and each flagged parent has a result of its own: a resultant above its constraint's threshold cannot enter
+      // the list), so the parents' selection stands as it is.  Matcher errors, candidates and pairs that may have several results are
+      // rendered; the others are counted.  Pairs that cannot be sorted -- no lazy path -- are all rendered.
+      const uint32_t m = res->n, C = (uint32_t)c->order.size();
+      const bool sorted = ordered ? lazy : hc.lazy;
+      std::vector<uint8_t> dead(b->n, 0);
+      bool any_dead = false;
+      for (uint32_t p : b->ex->par)
+        if (!obj_errs[p].empty()) dead[p] = 1, any_dead = true;   // (own review failed: no resultants; failed expansions have none anyway)
+      ResultantClasses rc;
+      rc.single = c->single_result.data();
+      rc.cls = cls.data();
+      rc.classes = (uint32_t)actions.size();
+      rc.nconstraints = C;
+      rc.parents = b->n;
+      rc.dead = any_dead ? dead.data() : nullptr;
+      ResultantSplit split;
+      float classify_ms = 0.f;
+      if (res_on_device) {
+        e->be->audit_resultants(res->dev.get(), res_fork.get(), rev, use_amb ? &rev_amb : nullptr, b->ex->par, b->ex->off_par, ranks, rc, split,
+                                &classify_ms);
+        a->select_ms += classify_ms;
+      } else {
+        GkResClassArgs ca{};
+        ca.viol = rev.viol.data();
+        ca.err = rev.err.data();
+        ca.amb = use_amb ? rev_amb.viol.data() : nullptr;
+        ca.single = rc.single;
+        ca.words = rev.words;
+        ca.nconstraints = C;
+        classify_resultants_host(ca, b->ex->par, b->ex->off_par, rc, [&](uint32_t p, uint32_t cc) { return !sorted || hc(p, cc); }, split);
+      }
+      uint64_t counted = 0, errors = 0;
+      for (uint32_t k = 0; k < rc.classes; ++k)
+        for (uint32_t cix = 0; cix < C; ++cix)
+          if (const uint64_t nc = split.counted[(size_t)k * C + cix]) {
+            const Constraint& con = *c->order[cix];
+            a->run.add_counted(con.kind + "/" + con.name, k ? actions[k] : con.action, nc);
+            counted += nc;
+          }
+      // the listed pairs as planes of their own, rendered as any batch's flagged pairs are (one parse per listed resultant)
+      BitPlane lv, le;
+      lv.assign((size_t)m * W, 0u);
+      le.assign((size_t)m * W, 0u);
+      for (size_t i = 0; i + 1 < split.render.size(); i += 2) {
+        const uint32_t r = split.render[i], cix = split.render[i + 1] & 0x7fffffffu, is_err = split.render[i + 1] >> 31;
+        (is_err ? le : lv)[(size_t)r * W + (cix >> 5)] |= 1u << (cix & 31u);
+        errors += is_err;
+      }
+      fold_resultant_results(a->run, *c, render(e, *c, *res, lv, le, rev.errlist, W, C, ep), children, ins);
+      const uint64_t rendered = split.render.size() / 2 - errors;
+      a->run.resultant_rendered += rendered;
+      a->run.resultant_counted += counted;
+      resultant_errors(obj_errs, res->host->obj_errors, children);
+      if (getenv("GK_TRACE_LAUNCH"))
+        fprintf(stderr, "[audit] %u resultants taken from the expanded batch: %llu pairs rendered, %llu counted, %llu matcher errors; sorted %s (%.3f ms on the device)\n",
+                m, (unsigned long long)rendered, (unsigned long long)counted, (unsigned long long)errors,
+                !sorted ? "no pair (every pair rendered)" : res_on_device ? "on the device" : "on the host", classify_ms);
+    } else if (!children.empty()) {
       const std::vector<gk_obj> cobjs = resultant_objs(children, ins);
       gk_result cres;
       memset(&cres, 0, sizeof cres);
@@ -1250,37 +1390,8 @@ static int audit_add(gk_audit_t* a, gk_batch_t* b, const char* ep_c, bool ordere
       }
       std::unique_ptr<ResultPriv> crp(static_cast<ResultPriv*>(cres.priv));
       cres.priv = nullptr;
-      struct Ident {
-        std::string g, v, k, ns, name;
-      };
-      std::unordered_map<uint32_t, Ident> ident;   // parents that have results from resultants
-      for (auto& v : crp->vio) {
-        const Child& ch = children[v.object];
-        auto it = ident.find(ch.parent);
-        if (it == ident.end()) {
-          Ident id2;
-          try {
-            VP po = json_parse(ins[ch.parent].json, ins[ch.parent].len);
-            split_gv(po, id2.g, id2.v, id2.k);
-            id2.ns = meta_str(po, "namespace");
-            id2.name = meta_str(po, "name");
-          } catch (JsonError&) {
-          }
-          it = ident.emplace(ch.parent, std::move(id2)).first;
-        }
-        const Constraint& con = *c->order[v.constraint];
-        StatusViolation sv;
-        sv.group = it->second.g, sv.version = it->second.v, sv.kind = it->second.k, sv.ns = it->second.ns, sv.name = it->second.name;
-        sv.message = ExpansionSystem::implied_by(ch.tmpl, v.msg);
-        sv.action = ch.action.empty() ? v.action : ch.action;   // OverrideEnforcementAction: the action only
-        sv.scoped_json = v.scoped_json;
-        a->run.fold(con.kind + "/" + con.name, std::move(sv));
-        a->run.results++;
-      }
-      // a resultant the review refused (manager.go:757-760 logs it and goes on): reported on its parent
-      for (size_t k = 0; k < crp->obj_errors.size() && k < children.size(); ++k)
-        if (!crp->obj_errors[k].empty() && obj_errs[children[k].parent].empty())
-          obj_errs[children[k].parent] = ExpansionSystem::implied_by(children[k].tmpl, crp->obj_errors[k]);
+      fold_resultant_results(a->run, *c, crp->vio, children, ins);
+      resultant_errors(obj_errs, crp->obj_errors, children);
     }
     a->run.add_object_errors(obj_errs);
   });
@@ -1291,6 +1402,13 @@ int gk_audit_add_batch(gk_audit_t* a, gk_batch_t* b, const char* ep, char** err)
 int gk_audit_add_batch_ordered(gk_audit_t* a, gk_batch_t* b, const char* ep, char** err) { return audit_add(a, b, ep, true, err); }
 
 float gk_audit_select_ms(gk_audit_t* a) { return a ? a->select_ms : 0.f; }
+
+int gk_audit_resultant_pairs(gk_audit_t* a, uint64_t* evaluated, uint64_t* counted) {
+  if (!a) return GK_ERR_INVALID;
+  if (evaluated) *evaluated = a->run.resultant_rendered;
+  if (counted) *counted = a->run.resultant_counted;
+  return GK_OK;
+}
 
 int gk_audit_export(gk_audit_t* a, char** buf, size_t* len, char** err) {
   if (!a || !buf || !len) return GK_ERR_INVALID;

@@ -53,4 +53,32 @@ GK_HD void gk_fold_parent(const GkFoldArgs& a, uint32_t j, Count&& count) {
   }
 }
 
+// The audit of an expanded batch (gk_audit_add_batch(_ordered)): the resultants' flagged pairs sorted into those the run counts and
+// those the host renders.  The CUDA backend runs it one thread per resultant (kernels.cu gk_res_classify_kernel), the host in loops.
+typedef struct {
+  const uint32_t* viol;          // the resultants' planes [resultants * words]
+  const uint32_t* err;
+  const uint32_t* amb;           // the resultants' ambiguity plane (bit clear: at most one result for the pair), or null: none
+  const uint8_t* single;         // [nconstraints] 1: one result for every pair of the constraint
+  uint32_t words, nconstraints;
+} GkResClassArgs;
+
+// resultant r, whose parent passes cand(c) when it can still enter constraint c's list: a matcher-error pair is emitted (emit(c, 1)); a
+// violation pair is emitted (emit(c, 0)) when its parent is a candidate or it may have several results, and counted (count(c)) otherwise
+template <class Cand, class Count, class Emit>
+GK_HD void gk_classify_resultant(const GkResClassArgs& a, uint32_t r, Cand&& cand, Count&& count, Emit&& emit) {
+  const uint32_t W = a.words;
+  for (uint32_t w = 0; w < W; ++w) {
+    const size_t at = (size_t)r * W + w;
+    const uint32_t v = a.viol[at], e = a.err[at], am = a.amb ? a.amb[at] : ~0u;
+    for (uint32_t b = v | e; b; b &= b - 1) {
+      const uint32_t k = gk_ctz32(b), c = w * 32u + k;
+      if (c >= a.nconstraints) continue;
+      if (e >> k & 1u) emit(c, 1u);
+      else if (cand(c) || !(a.single[c] || !(am >> k & 1u))) emit(c, 0u);
+      else count(c);
+    }
+  }
+}
+
 }  // namespace gk

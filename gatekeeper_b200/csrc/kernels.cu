@@ -282,6 +282,74 @@ __global__ void __launch_bounds__(256) gk_fold_kernel(GkFoldArgs a) {
     if (sh[C + c]) atomicAdd(a.err_totals + c, (unsigned long long)sh[C + c]);
   }
 }
+// ---- the audit of an expanded batch's resultants (Backend::audit_resultants)
+struct GkResAuditArgs {
+  GkResClassArgs a;
+  const uint32_t* par;             // the resident CSR of set_parents: parent par[j] has resultants off[j] .. off[j + 1] - 1
+  const uint32_t* off;
+  uint32_t m, nres;                // parents in the CSR, resultants
+  const uint32_t* rank;            // [parents] the parents' ranking (audit_candidates), and per constraint its threshold rank
+  const uint32_t* thr;
+  const uint8_t* cls;              // [nres] action class
+  const uint8_t* dead;             // [parents] or null
+  uint32_t classes;
+  unsigned long long* counted;     // [classes * nconstraints]
+  uint32_t* list;                  // [2 * cap] (resultant, constraint | is_err << 31)
+  uint32_t* nlist;
+  uint32_t cap;
+};
+// One thread per resultant row (fold_core.h gk_classify_resultant): a row is a few words, and a thread per row keeps the lanes busy
+// whatever the parents' fan-out -- a thread per parent would leave a warp waiting on its one parent with many resultants.  The parent
+// comes from a binary search of the resident CSR.  Counts go through shared memory [classes * C], one atomic per CTA and counter; each
+// warp reserves its pairs to render with one atomic (a first pass counts them, a second writes them).
+__global__ void __launch_bounds__(256) gk_res_classify_kernel(GkResAuditArgs x) {
+  extern __shared__ uint32_t sh[];
+  const uint32_t C = x.a.nconstraints, NC = x.classes * C, lane = threadIdx.x & 31u;
+  for (uint32_t i = threadIdx.x; i < NC; i += blockDim.x) sh[i] = 0;
+  __syncthreads();
+  for (uint32_t base = blockIdx.x * blockDim.x; base < x.nres; base += gridDim.x * blockDim.x) {   // (uniform per warp: the shuffles see all lanes)
+    const uint32_t r = base + threadIdx.x;
+    bool on = false;
+    uint32_t rk = 0;
+    if (r < x.nres) {
+      uint32_t lo = 0, hi = x.m;   // off[lo] <= r < off[hi]
+      while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (x.off[mid] <= r) lo = mid;
+        else hi = mid;
+      }
+      const uint32_t p = x.par[lo];
+      on = !(x.dead && x.dead[p]);
+      rk = x.rank[p];
+    }
+    auto cand = [&](uint32_t c) { return rk <= x.thr[c]; };
+    uint32_t ne = 0;
+    if (on) gk_classify_resultant(x.a, r, cand, [](uint32_t) {}, [&](uint32_t, uint32_t) { ++ne; });
+    uint32_t incl = ne;
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += t;
+    }
+    const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+    uint32_t at = 0;
+    if (lane == 31 && total) at = atomicAdd(x.nlist, total);
+    at = __shfl_sync(0xffffffffu, at, 31) + incl - ne;
+    if (on)
+      gk_classify_resultant(
+          x.a, r, cand, [&](uint32_t c) { atomicAdd(&sh[x.cls[r] * C + c], 1u); },
+          [&](uint32_t c, uint32_t is_err) {
+            if (at < x.cap) {
+              x.list[2 * (size_t)at] = r;
+              x.list[2 * (size_t)at + 1] = c | is_err << 31;
+            }
+            ++at;
+          });
+  }
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < NC; i += blockDim.x)
+    if (sh[i]) atomicAdd(x.counted + i, (unsigned long long)sh[i]);
+}
+
 // the fused exchange: the folded totals replace the ones the evaluation published to every peer
 __global__ void gk_fold_publish_kernel(GkFoldArgs a) {
   for (uint32_t c = threadIdx.x; c < a.nconstraints; c += blockDim.x)
@@ -1837,8 +1905,13 @@ class CudaBackend : public Backend {
   // by (group, version, kind); every object gets its triple's rank; the objects are merge-sorted by (that rank, namespace, name) and the
   // heads of equal runs scanned into one rank per identity.  Selection: per block of sorted positions and per constraint, the count of
   // flagged objects; per constraint (one warp), the rank of its limit-th flagged object; then every flagged bit at or below it.
+  // `keep`: the ranks and thresholds stay on the device, in a DevRanks, until the last copy of keep->dev is dropped.
+  struct DevRanks {
+    uint32_t* rank = nullptr;
+    uint32_t* thr = nullptr;
+  };
   void audit_candidates(void* b, const uint32_t* viol, uint32_t words, uint32_t C, uint32_t limit, const GvkOf& gvk_of, std::vector<uint32_t>& cand,
-                        float* device_ms) override {
+                        float* device_ms, AuditRanks* keep) override {
     auto* db = static_cast<DevBatch*>(b);
     std::lock_guard<std::mutex> l(mu_);
     CK(cudaSetDevice(device_));
@@ -1892,7 +1965,25 @@ class CudaBackend : public Backend {
     auto* gr = temps.take<uint32_t>((size_t)n * 4);
     auto* perm = temps.take<uint32_t>((size_t)n * 4);
     auto* head = temps.take<uint32_t>((size_t)n * 4);
-    auto* rank = temps.take<uint32_t>((size_t)n * 4);
+    uint32_t* rank = nullptr;
+    uint32_t* thr = nullptr;
+    if (keep) {
+      auto* kept = new DevRanks();
+      keep->dev = std::shared_ptr<void>(kept, [this](void* p) {
+        auto* k = static_cast<DevRanks*>(p);
+        cudaSetDevice(device_);
+        dfree(k->rank);
+        dfree(k->thr);
+        delete k;
+      });
+      dmalloc(&kept->rank, (size_t)n * 4);
+      dmalloc(&kept->thr, (size_t)C * 4);
+      rank = kept->rank;
+      thr = kept->thr;
+    } else {
+      rank = temps.take<uint32_t>((size_t)n * 4);
+      thr = temps.take<uint32_t>((size_t)C * 4);
+    }
     CK(cudaEventRecord(e2, stream_));
     if (m) {
       CK(cudaMemcpyAsync(d_list, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, stream_));
@@ -1910,7 +2001,6 @@ class CudaBackend : public Backend {
     gk_id_scatter_kernel<<<grid, T, 0, stream_>>>(perm, gr, n, rank);
     const uint32_t nb = (n + kSelChunk - 1) / kSelChunk;
     auto* cnt = temps.take<uint32_t>((size_t)nb * C * 4);
-    auto* thr = temps.take<uint32_t>((size_t)C * 4);
     auto* d_cand = temps.take<uint32_t>((size_t)n * words * 4);
     if ((size_t)C * 4 > max_smem_) throw BackendError{"audit candidates: too many constraints for one block's counters"};
     if ((size_t)C * 4 > 48 * 1024) CK(cudaFuncSetAttribute(gk_sel_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(C * 4)));
@@ -2232,6 +2322,77 @@ class CudaBackend : public Backend {
     a.totals = static_cast<unsigned long long*>(dst.totals);
     a.err_totals = static_cast<unsigned long long*>(dst.err_totals);
     launch_fold(a, st);
+  }
+
+  // The resultants' planes as eval() left them in `res` (and the ambiguity fork's in `amb`), the parents' CSR as set_parents() left it,
+  // the ranking audit_candidates() kept: gk_res_classify_kernel, then the counters and the listed pairs back to the host.  The list
+  // holds at most the resultants' flagged pairs, which their totals bound.
+  void audit_resultants(void* res, void* amb, const EvalOut& rev, const EvalOut* ramb, const std::vector<uint32_t>& par, const std::vector<uint32_t>& off,
+                        const AuditRanks& ranks, const ResultantClasses& cls, ResultantSplit& out, float* device_ms) override {
+    (void)ramb, (void)par, (void)off;   // (the planes and the CSR are read where they are resident)
+    auto* r = static_cast<DevBatch*>(res);
+    std::lock_guard<std::mutex> l(mu_);
+    CK(cudaSetDevice(device_));
+    const uint32_t C = cls.nconstraints, NC = cls.classes * C, m = r->n;
+    out.counted.assign(NC, 0);
+    out.render.clear();
+    if (device_ms) *device_ms = 0.f;
+    if (!m || !C) return;
+    auto* dr = static_cast<DevRanks*>(ranks.dev.get());
+    if (!dr) throw BackendError{"audit resultants: the parents' ranking was not kept on the device"};
+    if (r->fold_m + 1 != off.size() || (off.size() && off.back() != m)) throw BackendError{"audit resultants: the batch's parents are not the CSR given"};
+    if ((size_t)NC * 4 > max_smem_) throw BackendError{"audit resultants: too many constraints and action classes for one block's counters"};
+    uint64_t flagged = 0;
+    for (uint32_t c = 0; c < C && c < rev.totals.size(); ++c) flagged += rev.totals[c] + rev.err_totals[c];
+    if (flagged > 0x7fffffffull) throw BackendError{"audit resultants: more than 2^31 flagged pairs"};
+    Temps temps(this);
+    GkResAuditArgs x{};
+    x.a.viol = r->viol;
+    x.a.err = r->err;
+    x.a.amb = amb ? static_cast<DevBatch*>(amb)->viol : nullptr;
+    x.a.words = r->words;
+    x.a.nconstraints = C;
+    x.par = r->fold_par;
+    x.off = r->fold_off;
+    x.m = r->fold_m;
+    x.nres = m;
+    x.rank = dr->rank;
+    x.thr = dr->thr;
+    x.classes = cls.classes;
+    x.cap = (uint32_t)std::max<uint64_t>(flagged, 1);
+    auto* d_single = temps.take<uint8_t>(C);
+    auto* d_cls = temps.take<uint8_t>(m);
+    x.counted = temps.take<unsigned long long>((size_t)NC * 8);
+    x.list = temps.take<uint32_t>((size_t)x.cap * 8);
+    x.nlist = temps.take<uint32_t>(4);
+    CK(cudaMemcpyAsync(d_single, cls.single, C, cudaMemcpyHostToDevice, stream_));
+    CK(cudaMemcpyAsync(d_cls, cls.cls, m, cudaMemcpyHostToDevice, stream_));
+    if (cls.dead) {
+      auto* d_dead = temps.take<uint8_t>(cls.parents);
+      CK(cudaMemcpyAsync(d_dead, cls.dead, cls.parents, cudaMemcpyHostToDevice, stream_));
+      x.dead = d_dead;
+    }
+    x.a.single = d_single;
+    x.cls = d_cls;
+    CK(cudaMemsetAsync(x.counted, 0, (size_t)NC * 8, stream_));
+    CK(cudaMemsetAsync(x.nlist, 0, 4, stream_));
+    const size_t smem = (size_t)NC * 4;
+    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(gk_res_classify_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const uint32_t T = 256, grid = std::max(1u, std::min<uint32_t>((m + T - 1) / T, (uint32_t)sms_ * 8));
+    Event e0, e1;
+    CK(cudaEventRecord(e0, stream_));
+    gk_res_classify_kernel<<<grid, T, smem, stream_>>>(x);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(e1, stream_));
+    ++launches_;
+    uint32_t nl = 0;
+    CK(cudaMemcpyAsync(out.counted.data(), x.counted, (size_t)NC * 8, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaMemcpyAsync(&nl, x.nlist, 4, cudaMemcpyDeviceToHost, stream_));
+    CK(cudaStreamSynchronize(stream_));
+    if (nl > x.cap) throw BackendError{"audit resultants: more pairs to render than the resultants' totals"};
+    out.render.resize((size_t)nl * 2);
+    if (nl) CK(cudaMemcpy(out.render.data(), x.list, (size_t)nl * 8, cudaMemcpyDeviceToHost));
+    if (device_ms) CK(cudaEventElapsedTime(device_ms, e0, e1));
   }
 
  private:

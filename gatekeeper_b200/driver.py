@@ -73,6 +73,7 @@ EXPORTS = [
     "gk_audit_end", "gk_validation_messages", "gk_host_cpus", "gk_pin_host", "gk_blob_prefetch", "gk_coalescer_create", "gk_coalescer_review", "gk_coalescer_stats",
     "gk_coalescer_destroy", "gk_batch_size", "gk_batch_alg_bytes", "gk_batch_free", "gk_batch_refresh", "gk_batch_patch", "gk_free_result", "gk_free_str", "gk_dump",
     "gk_stat_description", "gk_audit_add_batch_ordered", "gk_audit_select_ms", "gk_audit_export", "gk_audit_merge",
+    "gk_audit_resultant_pairs",
 ]
 
 
@@ -125,6 +126,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.gk_audit_add_batch_ordered.argtypes = [P, P, S, PP]
     lib.gk_audit_select_ms.argtypes = [P]
     lib.gk_audit_select_ms.restype = C.c_float
+    lib.gk_audit_resultant_pairs.argtypes = [P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     lib.gk_audit_export.argtypes = [P, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), PP]
     lib.gk_audit_merge.argtypes = [P, C.c_char_p, C.c_size_t, PP]
     lib.gk_audit_report.argtypes = [P, PP]
@@ -610,6 +612,13 @@ class AuditRun:
     def select_ms(self) -> float:
         """Device time of the last add_batch_ordered's ranking and selection kernels (ms)."""
         return float(self.drv._lib.gk_audit_select_ms(self._a))
+
+    def resultant_pairs(self) -> tuple:
+        """(rendered, counted): the resultant violation pairs of expanded batches this run rendered on the host and counted from the
+        bitmap (matcher-error pairs are in neither; merged exports do not carry them)."""
+        ev, ct = C.c_uint64(), C.c_uint64()
+        self.drv._check(self.drv._lib.gk_audit_resultant_pairs(self._a, C.byref(ev), C.byref(ct)), C.c_char_p())
+        return ev.value, ct.value
 
     def export(self) -> bytes:
         """The run's partial state as an opaque, versioned byte string (merge() it into another run)."""

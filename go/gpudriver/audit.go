@@ -97,6 +97,16 @@ func (r *AuditRun) AddPageOrdered(b *C.gk_batch_t, enforcementPoint string) erro
 	return nil
 }
 
+// ResultantPairs returns the resultant violation pairs of expanded batches (GK_F_EXPAND) that this run rendered on the host and
+// counted from the bitmap (gk_audit_resultant_pairs): matcher-error pairs are in neither, and merged exports do not carry them.
+func (r *AuditRun) ResultantPairs() (evaluated, counted uint64, err error) {
+	var ev, ct C.uint64_t
+	if rc := C.gk_audit_resultant_pairs(r.a, &ev, &ct); rc != 0 {
+		return 0, 0, errors.New("gk_audit_resultant_pairs: invalid run")
+	}
+	return uint64(ev), uint64(ct), nil
+}
+
 // Export returns the run's partial state as an opaque versioned byte string (gk_audit_export), for Merge on another process.
 func (r *AuditRun) Export() ([]byte, error) {
 	var buf *C.char

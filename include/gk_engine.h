@@ -143,9 +143,10 @@ int gk_remove_constraint(gk_engine_t* e, const char* kind, const char* name);
  * kernel_ms and gpu_launches include the resultants and the fold.  The resultant planes belong to the batch: two device evaluations of
  * one expanded batch must not overlap (order them on one stream).  An expanded batch is refused by the eval calls once templates have
  * been added or removed since it was expanded ("ExpansionTemplates changed since the batch was expanded"); gk_batch_refresh expands
- * it again (a GK_F_KEEP_SOURCE blob batch from its kept device copy).  gk_audit_add_batch(_ordered) ignores the resultants: it
- * expands as for any batch.  Without GK_F_EXPAND these calls do not expand: while templates are registered they fail with a text
- * that says so, instead of returning rows in which the resultants' violations are missing. */
+ * it again (a GK_F_KEEP_SOURCE blob batch from its kept device copy).  gk_audit_add_batch(_ordered) takes an expanded batch's
+ * resultants from the batch while its templates are current: they are not expanded again on the host (see gk_audit_add_batch).
+ * Without GK_F_EXPAND these calls do not expand: while templates are registered they fail with a text that says so, instead of
+ * returning rows in which the resultants' violations are missing. */
 int gk_add_expansion_template(gk_engine_t* e, const char* json, size_t len, char** err);
 int gk_remove_expansion_template(gk_engine_t* e, const char* name);
 /* System.GetConflicts (pkg/expansion/system.go:81-83; db.go:62-70): the names of the stored ExpansionTemplates that are set aside
@@ -239,16 +240,27 @@ int gk_set_excluded_namespaces(gk_engine_t* e, const char* process, const char* 
 typedef struct gk_audit gk_audit_t;
 gk_audit_t* gk_audit_begin(gk_engine_t* e, uint32_t violations_limit, uint32_t msg_size, char** err);
 /* evaluate a resident batch at the enforcement point and fold every result into the run (messages are rendered for the
- * flagged pairs on all host cores) */
+ * flagged pairs on all host cores).  With ExpansionTemplates registered, every object is expanded and its resultants' results enter
+ * the run as the object's (see gk_add_expansion_template).  An EXPANDED batch (GK_F_EXPAND) whose templates have not changed since
+ * its upload or refresh brings its resultants: they are evaluated where they are resident, unfolded, and not expanded again.  Their
+ * pairs are sorted against the parents' candidates: a matcher error, a pair whose parent can still enter the constraint's list and a
+ * pair that may have several results are rendered; the other pairs, provably one result each, are counted.  The report is the one
+ * the same objects uploaded without GK_F_EXPAND give, counters included ("pairsEvaluated" / "pairsCounted" count the parents' own
+ * pairs).  A stale expanded batch, GK_AUDIT_EAGER, and a batch without the flag are expanded on the host as before. */
 int gk_audit_add_batch(gk_audit_t* a, gk_batch_t* b, const char* enforcement_point, char** err);
 /* gk_audit_add_batch with the candidates selected on the device, for a page of any mix of kinds (manager.go:886-945; the order is
  * SVQueue.Less, manager.go:117-137): the batch's objects are ranked by (group, version, kind, namespace, name) and, per constraint,
  * only the flagged objects at or below the `violations_limit`-th smallest identity (ties included) are rendered on the host; the
  * other pairs of constraints with one result per pair are counted from the bitmap.  The ambiguity netlist runs whatever the kinds.
- * The report equals gk_audit_add_batch's except for "pairsEvaluated" / "pairsCounted". */
+ * The report equals gk_audit_add_batch's except for "pairsEvaluated" / "pairsCounted".  An expanded batch's resultant pairs are
+ * sorted on the device as well, against the parents' ranking and thresholds. */
 int gk_audit_add_batch_ordered(gk_audit_t* a, gk_batch_t* b, const char* enforcement_point, char** err);
-/* device time (ms) of the ranking and selection of the last gk_audit_add_batch_ordered */
+/* device time (ms) of the ranking and selection of the last gk_audit_add_batch_ordered, and of the sorting of its resultant pairs */
 float gk_audit_select_ms(gk_audit_t* a);
+/* The resultant violation pairs of expanded batches (GK_F_EXPAND) that this run rendered on the host (*evaluated) and counted from
+ * the bitmap (*counted), over the batches added to it; matcher-error pairs, always rendered, are in neither.  Batches expanded on the
+ * host add nothing, and neither does gk_audit_merge: an export does not carry them.  Either pointer may be NULL. */
+int gk_audit_resultant_pairs(gk_audit_t* a, uint64_t* evaluated, uint64_t* counted);
 /* A sharded sweep (manager.go:886-945 over each shard, one updateConstraintStatus at the end: manager.go:984-1041).
  * gk_audit_export: the run's partial state -- per-constraint totals and status lists, per-action totals, object / result / pair
  * counters, object errors -- as an opaque versioned byte string in *buf (free with gk_free_str), *len bytes.
